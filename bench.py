@@ -7,19 +7,20 @@ bench.py -- BASELINE.json's metric: voxels/s warped (SpatialTransformer / interp
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...
     python bench.py --impl reference ...                           # CPU port of the reference, host cores
     python bench.py --op dice|cce|lc3d|resize|warp_mc|warp_slab|cfg5|mi|mi_segs|blur ...   # one op per line
+    python bench.py --dump-outputs DIR ...                         # also write the last timed step's output
 
 A "step" is one pass of the hot path over one batch: `--batch` (default 8) independent
 160x192x224x1 volumes with a random dense 3-channel flow U(-3,3) (configs[1] of
 BASELINE.json, SURVEY.md 8d), one kernel launch.  The batch's working set is 1.1 GB, far
-larger than the 126 MB L2, so no flush is needed between iterations.  At N GPUs every rank
+larger than the 50 MB L2 of an H100, so no flush is needed between iterations.  At N GPUs every rank
 warps its own batch (weak scaling, no data-path collective); `value` is whole-job
 voxels/s = N * batch * V * K / max-over-ranks device time (CUDA events, barrier + sync on
 both sides).
 
 JSON keys beyond the base contract:
   roofline     achieved = 20 B/voxel (12 flow + 4 source-once + 4 store, SURVEY.md 8d)
-               * voxels per launch / launch time; peak = MEASURED_PEAKS.json hbm_gbs.
-               `traffic` is the ncu dram__bytes of the committed capture (profiles/traffic.json, static).
+               * voxels per launch / launch time; peak = MEASURED_PEAKS.json hbm_gbs if present, else the
+               H100 SXM data-sheet 3.35 TB/s.
   long_run     the same launch timed over >= 200 steps (the K steps of the contract are only a few ms)
   e2e          the same metric through the public API with HOST (pinned) buffers: H2D of
                vol+flow and D2H of the result inside the timed region, every step.
@@ -30,6 +31,11 @@ JSON keys beyond the base contract:
   slab         (N > 1) ONE 160x192x224 volume sharded in z-slabs over the N ranks with the halo exchange
                (strong scaling): overlapped plan vs serial path, exchange-only and kernels-only times
   cfg5         (N > 1) BASELINE.json configs[4]: UNet fwd -> 16-channel warp -> Dice, batch-sharded and z-slab-sharded
+
+--dump-outputs DIR (headline warp, rank 0): after the K timed steps, the output of the last one is written as
+DIR/warp_out_item0.npy (batch item 0, [160,192,224,1] float32) and DIR/warp_out_sample.npy (4M elements of the whole
+[B,160,192,224,1] output at fixed seeded positions, float32).  The inputs come from a seeded device generator, so two
+builds run with the same arguments can be compared output for output.
 """
 import argparse
 import importlib.util
@@ -52,24 +58,13 @@ def measured_peak():
         with open(os.path.join(ROOT, 'MEASURED_PEAKS.json')) as f:
             return float(json.load(f)['hbm_gbs']), 'measured (MEASURED_PEAKS.json hbm_gbs)'
     except Exception:                                       # noqa: BLE001
-        return 6650.0, 'fallback (B200_PROFILING.md 6.65 TB/s)'
+        return 3350.0, 'fallback (H100 SXM data sheet, 3.35 TB/s)'
 
 
-def ncu_traffic(op):
-    """dram bytes per launch from the committed ncu summary, if present (profiles/traffic.json): a STATIC number
-    taken from the capture under profiles/, not a measurement of this run."""
-    try:
-        with open(os.path.join(ROOT, 'profiles', 'traffic.json')) as f:
-            return json.load(f).get(op)
-    except Exception:                                       # noqa: BLE001
-        return None
-
-
-def roofline(nbytes_per_step, ms_per_step, traffic_key, model, kernel=None):
+def roofline(nbytes_per_step, ms_per_step, model, kernel=None):
     peak, peak_src = measured_peak()
     achieved = nbytes_per_step / (ms_per_step * 1e-3) / 1e9
     r = {'bound': 'hbm', 'achieved': achieved, 'peak': peak, 'unit': 'GB/s', 'frac': achieved / peak,
-         'traffic': ncu_traffic(traffic_key), 'traffic_source': 'profiles/traffic.json (static, from the committed ncu capture)',
          'peak_source': peak_src, 'bytes_model': model, 'per': 'GPU'}
     if kernel:
         r['kernel'] = kernel
@@ -237,10 +232,9 @@ _CPU_READY = False
 def cpu_setup(orig_affinity=None):
     """One recipe for BOTH CPU legs (cpu_baseline of our arm and --impl reference): threads bound to cores
     (OMP_PROC_BIND=close, OMP_PLACES=cores -- must be in the environment before libgomp starts), as many threads as
-    the box gives this container -- min(cores in the affinity mask, cgroup CPU quota): the GPU boxes show 128 cores
-    but cap the container at 16 CPUs per 100 ms period, and 128 runnable threads get the whole group throttled for
-    the rest of a period (tools/cpu_leg_probe.py: 4.5 ms best, 94 ms median with 128 threads; 20.4-20.8 ms min-max
-    with 16) -- inputs first-touched by the OpenMP threads, the MEDIAN of >= 20 runs reported."""
+    the box gives this container -- min(cores in the affinity mask, cgroup CPU quota): a container may see many more
+    cores than its quota allows, and more runnable threads than the quota get the whole group throttled for the rest
+    of a period (bimodal timings) -- inputs first-touched by the OpenMP threads, the MEDIAN of >= 20 runs reported."""
     global _CPU_READY
     if orig_affinity:
         try:
@@ -324,7 +318,7 @@ def warp_config(args, world=1):
     return {'workload': warp_workload(args.batch, args.flow), 'batch_per_gpu': args.batch, 'volume': list(SHAPE),
             'channels': 1, 'interp_method': args.method,
             'parallelism': 'batch-sharded x%d, no collective' % world,
-            'l2': 'working set %.2f GB per step > 126 MB L2 (no flush needed)' % (20.0 * args.batch * V / 1e9)}
+            'l2': 'working set %.2f GB per step > 50 MB L2 (no flush needed)' % (20.0 * args.batch * V / 1e9)}
 
 
 def bench_reference(args):
@@ -392,8 +386,15 @@ def bench_warp(args):
         flow = torch.nn.functional.interpolate(coarse, size=SHAPE, mode='trilinear', align_corners=True)
         flow = (flow / flow.abs().amax() * 8).permute(0, 2, 3, 4, 1).contiguous()
     st = ne.layers.SpatialTransformer(interp_method=args.method, fill_value=None, halo=args.halo)
+    last = {}
+
+    def step():
+        last['out'] = st([vol, flow])
     sampler = ClockSampler(local).start()
-    ms = timed_region(lambda: st([vol, flow]), args.steps, args.warmup, world)
+    ms = timed_region(step, args.steps, args.warmup, world)
+    if args.dump_outputs and rank == 0:
+        dump_warp_outputs(args.dump_outputs, last.pop('out'))
+    last.clear()
     long_steps = max(args.steps, OPS_STEPS)
     ms_long = timed_region(lambda: st([vol, flow]), long_steps, 3, world, min_preheat_s=0.0)
     clocks = sampler.stop()
@@ -421,7 +422,7 @@ def bench_warp(args):
         'ms_per_step': ms / args.steps, 'higher_is_better': True, 'scaling': 'weak', 'vs_baseline': None,
         'dtype': 'f32', 'data': 'synthetic',
         'config': warp_config(args, world),
-        'roofline': roofline(bytes_per_launch, ms / args.steps, 'warp',
+        'roofline': roofline(bytes_per_launch, ms / args.steps,
                              '20 B/voxel = 12 flow + 4 source (each voxel once) + 4 store', 'warp3d_tile_kernel'),
         'long_run': {'steps': long_steps, 'ms_per_step': ms_long / long_steps,
                      'value': vox_per_step * long_steps / (ms_long * 1e-3),
@@ -462,6 +463,21 @@ def bench_warp(args):
     finish(world)
 
 
+DUMP_SAMPLE = 4 * 1024 * 1024
+
+
+def dump_warp_outputs(path, out):
+    """The headline's last output: batch item 0 in full and a fixed seeded sample of the whole batch (44 MB in all)."""
+    import numpy as np
+    import torch
+    os.makedirs(path, exist_ok=True)
+    np.save(os.path.join(path, 'warp_out_item0.npy'), out[0].float().cpu().numpy())
+    flat = out.reshape(-1)
+    g = torch.Generator().manual_seed(0)
+    idx = torch.randint(0, flat.numel(), (min(DUMP_SAMPLE, flat.numel()),), generator=g).to(flat.device)
+    np.save(os.path.join(path, 'warp_out_sample.npy'), flat[idx].float().cpu().numpy())
+
+
 def run_ops(args, world, rank, local, dev):
     """The other BASELINE.json configs inside the default line (driver-visible): compact records."""
     ops = {}
@@ -475,7 +491,7 @@ def run_ops(args, world, rank, local, dev):
             r = fn()
             ops[name] = {'workload': r['config']['workload'], 'metric': r['metric'], 'value': r['value'], 'unit': r['unit'],
                          'steps': r['steps'], 'ms_per_step': r['ms_per_step'],
-                         'roofline': {k: r['roofline'][k] for k in ('achieved', 'peak', 'frac', 'bytes_model', 'traffic', 'traffic_source')},
+                         'roofline': {k: r['roofline'][k] for k in ('achieved', 'peak', 'frac', 'bytes_model')},
                          'gpu_launches': r['gpu_launches'], 'clocks': r.get('clocks'), 'cpu_baseline': r.get('cpu_baseline')}
         except Exception as ex:                              # noqa: BLE001 -- one op must not take the headline down
             ops[name] = {'error': '%s: %s' % (type(ex).__name__, str(ex)[:300])}
@@ -519,8 +535,7 @@ def dice_record(args, world, rank, dev, cce=False):
                      elems * steps / (ms * 1e-3), 'elements/s', world, steps, args.warmup, ms, 'strong',
                      'BASELINE.json configs[2]: %s, y_true one-hot / y_pred softmax [4,160,192,224,16], voxel range sharded '
                      'over %d GPU(s) + all-reduce of [4,16,3] partial sums' % (name, world), {'l2': '3.5 GB read per step > L2'})
-    line['roofline'] = roofline(8.0 * (B * nz * SHAPE[1] * SHAPE[2] * L), ms / steps, 'cce' if cce else 'dice',
-                                '8 B per (voxel,label)', 'cce_vec4u_kernel<4,4>' if cce else 'dice_sums_vec4_kernel')
+    line['roofline'] = roofline(8.0 * (B * nz * SHAPE[1] * SHAPE[2] * L), ms / steps, '8 B per (voxel,label)', 'cce_vec4u_kernel<4,4>' if cce else 'dice_sums_vec4_kernel')
     line['gpu_launches'] = steps * (2 if cce else 3)
     line['clocks'] = clocks
     del t, p, lab
@@ -560,7 +575,7 @@ def lc3d_record(args, world, rank, dev, batch=None, cpu=True):
                      'BASELINE.json configs[3]: LocallyConnected3D 3x3x3, 16->16, input [%d,64,64,64,16], kernel '
                      '[238328,432,16] = 6.59 GB streamed once per step (> L2)' % B)
     line['roofline'] = roofline(4.0 * (P * F * Cout + B * I ** 3 * Cin + B * P * Cout + P * Cout), ms / steps,
-                                'lc3d' if B == 1 else ('lc3d_b8' if B == 8 else None), '4*(P*F*Cout + B*in + B*P*Cout + P*Cout)',
+                                '4*(P*F*Cout + B*in + B*P*Cout + P*Cout)',
                                 'lc3d_rows_kernel<4,2>' if B >= 8 else 'lc3d_patch_kernel')
     line['gpu_launches'] = steps
     line['clocks'] = clocks
@@ -593,7 +608,7 @@ def resize_record(args, world, rank, dev):
     line = base_line('output voxels/s, Resize zoom 2 of a half-resolution 3-ch flow to 160x192x224',
                      world * B * V * steps / (ms * 1e-3), 'voxels/s', world, steps, args.warmup, ms, 'weak',
                      'Resize(2) on [%d,80,96,112,3] (reference models.py:803-804)' % B)
-    line['roofline'] = roofline(4.0 * 3 * B * V * (1 + 1 / 8), ms / steps, 'resize', '4C/z^3 + 4C per output voxel',
+    line['roofline'] = roofline(4.0 * 3 * B * V * (1 + 1 / 8), ms / steps, '4C/z^3 + 4C per output voxel',
                                 'resize3d_kernel')
     line['gpu_launches'] = steps
     line['clocks'] = clocks
@@ -636,7 +651,7 @@ def warp_mc_record(args, world, rank, dev, C=None):
                      world * B * V * steps / (ms * 1e-3), 'voxels/s', world, steps, args.warmup, ms, 'weak',
                      'SpatialTransformer warp of [%d,160,192,224,%d] fp32 (the %d-label softmax of BASELINE.json configs[4]), '
                      'random dense flow %s' % (B, C, C, 'U(-3,3) i.i.d.' if args.flow == 'iid' else 'smooth, max|u|=3'))
-    line['roofline'] = roofline((12.0 + 8.0 * C) * B * V, ms / steps, 'warp_c%d' % C,
+    line['roofline'] = roofline((12.0 + 8.0 * C) * B * V, ms / steps,
                                 '12 flow + 4C source (each voxel once) + 4C store per voxel', 'warp3d_march_kernel')
     line['gpu_launches'] = steps
     line['clocks'] = clocks
@@ -846,7 +861,7 @@ def bench_mi(args, segs=False):
                          'MutualInformation(nb_bins=16).%s on %d x 160x192x224 (reference metrics.py:41-336); '
                          'min/max + histogram + combine + finalise kernels per step' % ('segs, 16 labels' if segs else 'volumes', B))
         line['dtype'] = 'f32 (3xTF32 tensor-core contraction)'
-        line['roofline'] = roofline(per_voxel * B * V, ms / args.steps, 'mi_segs' if segs else 'mi',
+        line['roofline'] = roofline(per_voxel * B * V, ms / args.steps,
                                     '%d B/voxel (two fp32 %s read once; the quantised [V,16] maps never exist)'
                                     % (per_voxel, 'maps' if segs else 'volumes'), kern)
         if not segs:
@@ -884,7 +899,7 @@ def bench_blur(args):
                          world * B * V * args.steps / (ms * 1e-3), 'voxels/s', world, args.steps, args.warmup, ms, 'weak',
                          'GaussianBlur(sigma=%g) on [%d,160,192,224,1] (reference layers.py:251-364): three separable passes'
                          % (args.sigma, B))
-        line['roofline'] = roofline(8.0 * B * V, ms / args.steps, 'blur',
+        line['roofline'] = roofline(8.0 * B * V, ms / args.steps,
                                     '8 B/voxel for the whole blur (read once, write once); the three-pass path moves '
                                     '24 B/voxel, so 0.33 is its ceiling', 'sepconv_col4_kernel x2 + sepconv_row_kernel')
         line['gpu_launches'] = args.steps * 3
@@ -941,7 +956,11 @@ def main():
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--no-numpy-baseline', action='store_true')
     ap.add_argument('--no-extras', action='store_true', help='headline only: no ops / slab / cfg5 sub-records')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write the output of the last timed step of the headline warp as DIR/*.npy')
     args = ap.parse_args()
+    if args.dump_outputs and (args.op != 'warp' or args.impl != 'ours'):
+        raise SystemExit('bench.py: --dump-outputs writes the headline warp (--op warp) of this implementation only')
     if args.impl == 'reference':
         return bench_reference(args)
     import torch

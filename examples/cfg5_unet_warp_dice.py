@@ -15,7 +15,7 @@ kernels (z-marching ring kernel, nrt_warp_march.cu; dice_sums kernels, nrt_metri
 
   --mode batch   the global batch is split over the ranks; every rank pushes its own volumes through
                  UNet -> warp -> Dice; the only collective is the all-reduce of the scalar mean loss.
-  --mode slab    "8xB200 z-slab shard with halo": EVERY volume of the global batch is split along z over the
+  --mode slab    "8xH100 z-slab shard with halo": EVERY volume of the global batch is split along z over the
                  ranks.  A rank runs the UNet on its slab plus the network's receptive-field margin (24 planes,
                  windows aligned to the pooling stride 8, so the slab's segmentation equals the whole-volume
                  one), keeps only its own planes, exchanges `halo` planes of the 16-channel segmentation with

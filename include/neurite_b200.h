@@ -1,5 +1,5 @@
 /*
- * neurite_b200.h -- C ABI of libneurite_b200.so (hand-written CUDA for sm_100a).
+ * neurite_b200.h -- C ABI of libneurite_b200.so (hand-written CUDA for sm_90a).
  *
  * The reference (adalca/neurite @ 7c4b05e) has no FFI: its extension boundary is python
  * callables / Keras layers over TensorFlow ops (SURVEY.md 8b).  Each entry point below
@@ -41,7 +41,7 @@ typedef enum {
   NRT_E_SIZE = -2,    /* size outside what the kernels index (int32 per batch item)    */
   NRT_E_LAUNCH = -3,  /* CUDA launch / runtime error (string has cudaGetErrorString)   */
   NRT_E_ALIGN = -4,   /* pointer not aligned as the entry point requires               */
-  NRT_E_NODEV = -5    /* no usable sm_100 device / driver                              */
+  NRT_E_NODEV = -5    /* no usable sm_90 device / driver                               */
 } nrt_status;
 
 enum { NRT_LINEAR = 0, NRT_NEAREST = 1 };

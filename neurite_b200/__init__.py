@@ -1,5 +1,5 @@
 """
-neurite_b200 -- B200-native (sm_100a) implementation of neurite's per-volume hot path:
+neurite_b200 -- H100-native (sm_90a) implementation of neurite's per-volume hot path:
 interpn / resize / SpatialTransformer, LocallyConnected3D, Dice and the label-weighted
 categorical cross-entropy, behind neurite's own call signatures.
 

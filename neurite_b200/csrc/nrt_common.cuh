@@ -1,4 +1,4 @@
-// nrt_common.cuh -- shared host/device helpers for libneurite_b200 (sm_100a only).
+// nrt_common.cuh -- shared host/device helpers for libneurite_b200 (sm_90a: TMA, mbarrier).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -7,8 +7,8 @@
 
 #include "../../include/neurite_b200.h"
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "libneurite_b200 is written for sm_100a (B200) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 900)
+#error "libneurite_b200 needs sm_90a (H100): TMA tensor loads and mbarrier transaction counts"
 #endif
 
 namespace nrt {

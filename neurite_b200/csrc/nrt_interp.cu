@@ -1,4 +1,4 @@
-// nrt_interp.cu -- N-D gridded interpolation for sm_100a:
+// nrt_interp.cu -- N-D gridded interpolation for sm_90a:
 //   nrt_interpn_f32  (explicit loc tensor)      reference utils.py:73-220
 //   nrt_warp_f32     (identity grid + flow)     voxelmorph SpatialTransformer contract
 //   nrt_resize_f32   (in-kernel linspace grid)  reference utils.py:223-265, layers.py:154-181
@@ -164,8 +164,7 @@ resize3d_kernel(const float* __restrict__ vol, float* __restrict__ out, ResizeGe
   // shared memory so that the row leaves as three fully coalesced 128-byte stores instead of
   // three 12-byte-strided ones (3x fewer L2 write sectors).  All lanes of a row take part, so
   // lanes past the x end keep running on the zero table entry (offset 0, weights 0).
-  // (measured on B200: 0.350 ms with the exchange vs 0.317 ms without -- the two warp syncs cost more than
-  //  the saved write sectors -- so the exchange is compiled out)
+  // (compiled out: the two warp syncs cost more than the write sectors they save)
   constexpr bool kRowStore = false && (METHOD == NRT_LINEAR && CT == 3);
   __shared__ float s_row[kRowStore ? 8 * 96 : 1];
   if (oy >= w.M[1] || (!kRowStore && ox >= w.M[2])) return;
@@ -294,18 +293,16 @@ resize3d_kernel(const float* __restrict__ vol, float* __restrict__ out, ResizeGe
 // ---------------------------------------------------------------------------------------
 // resize3d_tile_kernel: the linear z-marching kernel with its SOURCE staged in shared memory.  resize3d_kernel issues
 // its corner loads to L1/L2 when an output plane enters a new source cell and then waits ~600 cycles for them with
-// 3 CTAs per SM: it is latency-bound (74 % issue-active, 0.43 of the roofline; a packed two-voxel variant that
-// halves the arithmetic is no faster).  An up-sampling zoom reads a SMALL source box per output tile -- 32 x 8 x 32
+// 3 CTAs per SM: it is latency-bound.  An up-sampling zoom reads a SMALL source box per output tile -- 32 x 8 x 32
 // outputs of a x2 zoom touch 18 x 6 x 18 source voxels -- so the CTA fetches that box with ONE TMA tensor load
 // (coordinates from the tile's own table entries, extents = the largest box any tile needs, computed on the host
 // with the same fp32 linspace arithmetic) and every corner read becomes a ~30-cycle LDS.
 // A tile whose box would not fit the staged extents (cannot happen when host and device agree) or a zoom whose
 // boxes are larger than the budget (down-sampling) takes resize3d_kernel.
 // ---------------------------------------------------------------------------------------
-// packed fp32x2 arithmetic (pack2 / fma2 in nrt_interp.cuh; FFMA2 issues at the scalar FFMA rate on sm_100: two results
-// per issue slot).  Bit-exactness: ptxas fuses mul.f32x2 + add.f32x2 into one FFMA2 (single rounding) even with
-// fmad=false, so the reference's separately rounded ops are written as  a*b = fma(a, b, -0)  and  a+b = fma(a, 1, b)
-// with the identity operands (-0,-0) and (1,1) passed as kernel PARAMETERS (visible constants are folded and re-fused).
+// fp32 pair arithmetic (pack2 / fma2 in nrt_interp.cuh).  Bit-exactness: the reference's separately rounded ops are
+// written as  a*b = fma(a, b, -0)  and  a+b = fma(a, 1, b)  with the identity operands (-0,-0) and (1,1) passed as
+// kernel PARAMETERS (visible constants would be folded and the multiply and add re-fused into one rounding).
 struct ResizeBox { int bz, by, bx; };            // staged source extents (bx already padded for the TMA alignment)
 
 template <int CT, int TZ>
@@ -447,11 +444,10 @@ resize3d_tile_kernel(const __grid_constant__ CUtensorMap tm_vol, const float* __
 }
 
 // ---------------------------------------------------------------------------------------
-// resize3d_pair_kernel: the packed voxel-pair kernel, second version: the three things the first version's SASS and capture
-// (profiles/r02_ncu_full_resize.txt: 83 instructions per voxel, issue-bound) showed to be overhead removed:
-//   * corner reads are LDS with 32-bit offsets and immediate channel offsets.  The first packed kernel (round 2,
-//     removed) read through a pointer that is shared OR global at run time, i.e. generic LD.E with 64-bit address
-//     arithmetic: 88 instructions per 24 loads.  Here the marching loop is a template on the address space.
+// resize3d_pair_kernel: the voxel-pair kernel (two x positions per thread share the table reads and the z / y weights):
+//   * corner reads are LDS with 32-bit offsets and immediate channel offsets, not generic loads through a pointer that
+//     is shared OR global at run time (64-bit address arithmetic per load): the marching loop is a template on the
+//     address space.
 //   * the two source planes of a z cell live in two register sets tagged with the source plane they hold; entering
 //     the next cell loads ONE plane into the set that is free and swaps the roles of the sets (two copies of the
 //     arithmetic, selected by a CTA-uniform branch) instead of moving 24 registers from `hi` to `lo`.
@@ -459,10 +455,7 @@ resize3d_tile_kernel(const __grid_constant__ CUtensorMap tm_vol, const float* __
 //     monotonic: no loop over the table, no second block barrier) and issues the TMA load while the other threads
 //     build the tables; no dynamically indexed kernel parameters (they cost a 128-byte local-memory copy per thread).
 // Same arithmetic and rounding order as resize3d_tile_kernel (bit-exact with the oracle); two x positions per thread
-// are the halves of packed fp32x2 registers.
-// Tried on top and dropped (profiles/README.md): a persistent CTA with two box buffers that prefetches the next tile's
-// box (the wait for the box is 16.5 % of the warp samples here).  Correct, but the extra loop state does not fit the
-// 128 registers that 2 CTAs per SM allow: spill reloads inside the plane loop, 0.247 ms against 0.166.
+// are the halves of fp32 register pairs.
 // ---------------------------------------------------------------------------------------
 __device__ __forceinline__ Axis resize_axis(int S, int M, float delta, int i) {
   // tf.linspace(0, S-1, M): endpoints exact, interior 0 + delta*i  (utils.py:259)
@@ -965,10 +958,8 @@ warp3d_tile_kernel(const __grid_constant__ CUtensorMap tm_vol,
   // instruction (three REDUX instead of fifteen shuffle + add steps).  A large coherent displacement means the
   // speculative box is useless; the box is then re-staged around the displaced position, so that the halo only has
   // to cover the variation of the flow inside the tile.  An incoherent flow averages out and keeps the box.
-  // (Measured, profiles/: every warp doing this redundantly costs 12 % on the BASELINE workload -- 8 x 60
-  // instructions per tile are ~9 % of the tile's instruction count -- one warp + one block barrier costs 2-2.6 %.
-  // Handing the decision over through a third mbarrier instead of the block barrier, so that warps 1-7 never wait for
-  // the flow tile, measured the same: 0.2220 vs 0.2177 ms with following off, same box.)
+  // (Every warp doing this redundantly would add 8 x 60 instructions per tile, ~9 % of the tile's instruction count;
+  // one warp + one block barrier is far cheaper.)
   int sz = 0, sy = 0, sx = 0;
   if (follow) {                                      // launch-uniform
     if (threadIdx.x < 32) {
@@ -1359,8 +1350,8 @@ static int try_tile_path(const float* vol, const float* flow, float* out, int B,
   const int H = shape[1], W = shape[2];
   if (env_int("NRT_WARP_TILE", 1) == 0) return NRT_OK;
   if (W % 4 != 0 || !aligned16(vol) || !aligned16(flow) || !aligned16(out) || W < 32) return NRT_OK;
-  // tile shapes (TZ x TY x 32) and halos built: the default 8x8x32 runs 4 CTAs per SM (best
-  // measured on B200, profiles/); `halo` picks the smallest built halo that covers it.
+  // tile shapes (TZ x TY x 32) and halos built: the default 8x8x32 runs 4 CTAs per SM;
+  // `halo` picks the smallest built halo that covers it.
   // 2: 8x8x32 (default), 3: 4x8x32
   int cfg = env_int("NRT_WARP_TILE_CFG", 2);
   if (cfg != 2 && cfg != 3) cfg = 2;
@@ -1499,9 +1490,8 @@ static int warp_impl(const float* vol, const float* flow, float* out, int B, con
               (obs == 0 || obs >= plane * out_n0 * C), NRT_E_ARG, "batch stride smaller than one batch item");
   if (B == 0 || out_n0 == 0) return NRT_OK;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  // 3 or more channels: z-marching ring kernel (all channels of a voxel side by side in shared memory).  Measured on
-  // B200 (profiles/r02_sweep_visit1.txt, i.i.d. / smooth flows): C = 3: 0.48 / 0.59 vs 0.39 / 0.42 for the box-tile
-  // kernel, C = 4: 0.56 / 0.68 vs 0.47 / 0.53; C = 2 stays on the box tiles (0.54 / 0.65 vs 0.50 / 0.53).
+  // 3 or more channels: z-marching ring kernel (all channels of a voxel side by side in shared memory); C = 2 stays
+  // on the box tiles, whose halo is still small at two channels.
   const int march_min_c = env_int("NRT_MARCH_SMALLC", 0) ? 2 : env_int("NRT_MARCH_MINC", 3);
   if (D == 3 && C >= 2 && C >= march_min_c) {
     bool used = false;
@@ -1569,8 +1559,8 @@ int nrt_resize_f32(const float* vol, float* out, int B, const int32_t* in_shape,
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (D == 3 && in_vox * C <= 0x7fffffffLL && getenv("NRT_RESIZE_GENERIC") == nullptr) {
     const char* tze = getenv("NRT_RESIZE_TZ");
-    // planes per CTA: 32 measured best on B200 (0.261 ms vs 0.318 at 8 for Resize(2) of [8,80,96,112,3]); short
-    // slabs take fewer so that the grid keeps a few waves
+    // planes per CTA: 32 (fewer prologues and box waits per output plane); short slabs take fewer so that the grid
+    // keeps a few waves
     int TZ = tze ? atoi(tze) : (out_n0 >= 64 ? 32 : (out_n0 >= 24 ? 16 : 8));
     if (TZ != 16 && TZ != 32 && TZ != 64) TZ = 8;
     if (method != NRT_LINEAR || C < 1 || C > 4) TZ = 8;          // the marching path is linear, C = 1..4
@@ -1589,7 +1579,6 @@ int nrt_resize_f32(const float* vol, float* out, int B, const int32_t* in_shape,
       bxs.by = resize_axis_extent(rg.g.S[1], rg.M[1], rg.delta[1], 0, rg.M[1], tyt, 1);
       bxs.bx = resize_axis_extent(rg.g.S[2], rg.M[2], rg.delta[2], 0, rg.M[2], 32, xalign);
       bxs.bx = (bxs.bx + xalign - 1) / xalign * xalign;
-      // (64 planes per CTA -- half the prologues and box waits, an 82 KB box -- measured slower than 32: 0.172 vs 0.166 ms)
       const int tzt = (TZ == 64) ? 32 : TZ;
       bxs.bz = resize_axis_extent(rg.g.S[0], rg.M[0], rg.delta[0], out_z0, out_n0, tzt, 1);
       const size_t box_bytes = (size_t)bxs.bz * bxs.by * bxs.bx * C * 4;

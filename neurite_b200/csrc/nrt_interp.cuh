@@ -216,9 +216,10 @@ struct BoxBounds { int lo_z, hi_z, lo_y, hi_y, lo_x, hi_x; };
 // last_stride_elems != 0: element stride of the LAST dimension (batch items not densely packed; multiple of 4)
 int encode_f32_tiled(CUtensorMap* tm, const void* base, int rank, const uint64_t* dims, const uint32_t* box,
                      uint64_t last_stride_elems = 0);
-// packed fp32x2 arithmetic: two results per issue slot (fma.rn.f32x2).  The reference's separately rounded products and
-// sums are written as a*b = fma(a, b, -0) and a+b = fma(a, 1, b), identity operands passed as kernel parameters
-// (see nrt_interp.cu, resize3d kernels, for why).
+// fp32 pairs: two values in one 64-bit register pair, so that a kernel can carry two voxels through one code path.
+// sm_90 has no packed fp32 FMA: fma2 issues two scalar single-rounding FMAs.  The reference's separately rounded
+// products and sums are written as a*b = fma(a, b, -0) and a+b = fma(a, 1, b), identity operands passed as kernel
+// parameters (see nrt_interp.cu, resize3d kernels, for why).
 typedef unsigned long long f32x2;
 __device__ __forceinline__ f32x2 pack2(float a, float b) {
   f32x2 r;
@@ -229,9 +230,9 @@ __device__ __forceinline__ void unpack2(f32x2 v, float& a, float& b) {
   asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v));
 }
 __device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) {
-  f32x2 r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-  return r;
+  float a0, a1, b0, b1, c0, c1;
+  unpack2(a, a0, a1); unpack2(b, b0, b1); unpack2(c, c0, c1);
+  return pack2(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
 
 

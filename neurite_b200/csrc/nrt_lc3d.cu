@@ -1,4 +1,4 @@
-// nrt_lc3d.cu -- LocallyConnected3D (implementation 1) forward for sm_100a.
+// nrt_lc3d.cu -- LocallyConnected3D (implementation 1) forward for sm_90a.
 // Reference: neurite/tf/layers.py:1126-1197 (local_conv), :1098-1101 (bias, activation).
 //
 // The layer is a weight STREAM: every output position owns a private F x Cout block
@@ -70,10 +70,7 @@ __device__ __forceinline__ int64_t patch_origin(const LcGeo& g, int64_t p) {
 constexpr int kLcMaxWarps = 7;              // consumer groups (<= ring slots - 1) + 1 producer warp
 constexpr int kLcMaxStages = 8;
 
-// P2: the 4 x BB accumulators are updated with packed fma.rn.f32x2 (two fused multiply-adds per issue slot on
-// sm_100): the weight pairs are the halves of the LDS.128 result, the input value is broadcast to both halves.
-// Bit-identical to the scalar chain (the same fused operation per accumulator).
-template <int BB, int WPP, bool P2 = false>
+template <int BB, int WPP>
 __global__ void __launch_bounds__((kLcMaxWarps * WPP + 1) * 32, 1)
 lc3d_stream_kernel(const float* __restrict__ x, const float* __restrict__ kernel,
                    const float* __restrict__ bias, float* __restrict__ out, LcGeo g, int b_base,
@@ -137,9 +134,8 @@ lc3d_stream_kernel(const float* __restrict__ x, const float* __restrict__ kernel
     const uint32_t ph = (uint32_t)((k / stages) & 1);
     const float* xp = x + (int64_t)b0 * g.x_batch + patch_origin(g, g.p0 + n);
     float acc[BB][4];
-    unsigned long long acc2[BB][2];                           // P2: (acc0, acc1), (acc2, acc3) as packed pairs
 #pragma unroll
-    for (int b = 0; b < BB; ++b) { acc[b][0] = acc[b][1] = acc[b][2] = acc[b][3] = 0.f; acc2[b][0] = acc2[b][1] = 0ull; }
+    for (int b = 0; b < BB; ++b) acc[b][0] = acc[b][1] = acc[b][2] = acc[b][3] = 0.f;
     const float4* w4 = reinterpret_cast<const float4*>(smem_raw + (size_t)slot * blk_stride);
     for (int i0 = 0; i0 < iters; i0 += CH) {
       float xv[CH][BB];
@@ -158,42 +154,20 @@ lc3d_stream_kernel(const float* __restrict__ x, const float* __restrict__ kernel
 #pragma unroll
       for (int c = 0; c < CH; ++c) {
         const int i = lane + ((i0 + c) << 5);
-        {
-          // past the end of the block the weights are zero (no branch: the packed accumulators stay in place)
-          const float4 wv = (i < n4) ? w4[i] : make_float4(0.f, 0.f, 0.f, 0.f);
-          if (P2) {
-            unsigned long long w01, w23;
-            asm("mov.b64 %0, {%1, %2};" : "=l"(w01) : "f"(wv.x), "f"(wv.y));
-            asm("mov.b64 %0, {%1, %2};" : "=l"(w23) : "f"(wv.z), "f"(wv.w));
+        // past the end of the block the weights are zero (no branch: the accumulators stay in place)
+        const float4 wv = (i < n4) ? w4[i] : make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
-            for (int b = 0; b < BB; ++b) {
-              unsigned long long xx;
-              asm("mov.b64 %0, {%1, %1};" : "=l"(xx) : "f"(xv[c][b]));
-              asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc2[b][0]) : "l"(xx), "l"(w01));
-              asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc2[b][1]) : "l"(xx), "l"(w23));
-            }
-          } else {
-#pragma unroll
-            for (int b = 0; b < BB; ++b) {
-              acc[b][0] = fmaf(xv[c][b], wv.x, acc[b][0]);
-              acc[b][1] = fmaf(xv[c][b], wv.y, acc[b][1]);
-              acc[b][2] = fmaf(xv[c][b], wv.z, acc[b][2]);
-              acc[b][3] = fmaf(xv[c][b], wv.w, acc[b][3]);
-            }
-          }
+        for (int b = 0; b < BB; ++b) {
+          acc[b][0] = fmaf(xv[c][b], wv.x, acc[b][0]);
+          acc[b][1] = fmaf(xv[c][b], wv.y, acc[b][1]);
+          acc[b][2] = fmaf(xv[c][b], wv.z, acc[b][2]);
+          acc[b][3] = fmaf(xv[c][b], wv.w, acc[b][3]);
         }
       }
     }
     __syncwarp();
     if (lane == 0) {                             // slot free: every lane has read its share
       asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(smem_u32(empty + slot)) : "memory");
-    }
-    if (P2) {
-#pragma unroll
-      for (int b = 0; b < BB; ++b) {
-        asm("mov.b64 {%0, %1}, %2;" : "=f"(acc[b][0]), "=f"(acc[b][1]) : "l"(acc2[b][0]));
-        asm("mov.b64 {%0, %1}, %2;" : "=f"(acc[b][2]), "=f"(acc[b][3]) : "l"(acc2[b][1]));
-      }
     }
     // fold the 32/CQ lanes that share an output quad
 #pragma unroll
@@ -219,8 +193,8 @@ lc3d_stream_kernel(const float* __restrict__ x, const float* __restrict__ kernel
 
 // ---------------------------------------------------------------------------------------
 // patch kernel (batch > 1).  lc3d_stream_kernel gathers a position's input patch lane by lane from L2: at
-// batch 8 that is 216 scalar loads per lane and ~6 integer instructions of addressing each -- 7100 warp
-// instructions per position, ALU pipe 62 % busy, 0.42 of the HBM roofline (profiles/r01_ncu_full_lc3d_b8.txt).
+// batch 8 that is 216 scalar loads per lane and ~6 integer instructions of addressing each -- ~7100 warp
+// instructions per position, which keeps the ALU pipe busy instead of the weight stream.
 // Here the producer thread fetches the patch with ONE TMA tensor load per position -- the box
 // (Cin, K2, K1, K0, NB) of the channels-last input [B, I0, I1, I2, Cin] lands in shared memory as [b][j] with
 // exactly the reference's feature order j = ((i0*K1 + i1)*K2 + i2)*Cin + c (layers.py:1173-1188) -- on the same
@@ -276,16 +250,16 @@ lc3d_patch_kernel(const __grid_constant__ CUtensorMap tm_x, const float* __restr
     const unsigned char* base = smem_raw + (size_t)slot * slot_stride;
     const float4* w4 = reinterpret_cast<const float4*>(base);
     const float* sx = reinterpret_cast<const float*>(base + patch_off) + (size_t)sub * BB * g.F;
-    unsigned long long acc2[BB][2];
+    float acc[BB][4];
 #pragma unroll
-    for (int b = 0; b < BB; ++b) acc2[b][0] = acc2[b][1] = 0ull;
+    for (int b = 0; b < BB; ++b) acc[b][0] = acc[b][1] = acc[b][2] = acc[b][3] = 0.f;
     // Parity aliasing guard.  A group visits only every `groups`-th step, so it may reach for step k while the PREVIOUS
     // use of this slot (step k - stages, another group's) is still in flight: copies of different steps can complete
     // out of order (the patch comes through the tensor path, the weights through the bulk path), the barrier would
     // still be one phase behind and try_wait on the next parity would return at once -- on a half-filled slot.
     // First make sure the previous round of the slot has been CONSUMED (which implies it had landed); the `empty`
     // barrier cannot be more than one phase away from what this warp expects, so that wait cannot alias.
-    // (Found on B200 as a 4 s mbarrier timeout at full size, batch 2 -- never with the sanitizer's slower timing.)
+    // (Seen as a 4 s mbarrier timeout at full size, batch 2 -- never with the sanitizer's slower timing.)
     if (k >= stages) mbar_wait(empty + slot, ph ^ 1u, 2000000 + k);
     mbar_wait(full + slot, ph, k);
     // lane l reads float4 l, l+32, ... of the weight block: patch feature j = i / CQ advances by 32 / CQ per step
@@ -294,15 +268,12 @@ lc3d_patch_kernel(const __grid_constant__ CUtensorMap tm_x, const float* __restr
     const int xstep = 32 >> cq_log2;
 #define NRT_LC_STEP(WV, XP)                                                                              \
     do {                                                                                                 \
-      unsigned long long w01, w23;                                                                       \
-      asm("mov.b64 %0, {%1, %2};" : "=l"(w01) : "f"((WV).x), "f"((WV).y));                               \
-      asm("mov.b64 %0, {%1, %2};" : "=l"(w23) : "f"((WV).z), "f"((WV).w));                               \
       _Pragma("unroll") for (int b = 0; b < BB; ++b) {                                                   \
         const float xv = (XP)[b * g.F];                                                                  \
-        unsigned long long xx;                                                                           \
-        asm("mov.b64 %0, {%1, %1};" : "=l"(xx) : "f"(xv));                                               \
-        asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc2[b][0]) : "l"(xx), "l"(w01));                      \
-        asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc2[b][1]) : "l"(xx), "l"(w23));                      \
+        acc[b][0] = fmaf(xv, (WV).x, acc[b][0]);                                                         \
+        acc[b][1] = fmaf(xv, (WV).y, acc[b][1]);                                                         \
+        acc[b][2] = fmaf(xv, (WV).z, acc[b][2]);                                                         \
+        acc[b][3] = fmaf(xv, (WV).w, acc[b][3]);                                                         \
       }                                                                                                  \
     } while (0)
     const int full_iters = n4 >> 5;
@@ -318,12 +289,6 @@ lc3d_patch_kernel(const __grid_constant__ CUtensorMap tm_x, const float* __restr
 #undef NRT_LC_STEP
     __syncwarp();
     if (lane == 0) mbar_arrive(empty + slot);      // slot free: every lane has read its share
-    float acc[BB][4];
-#pragma unroll
-    for (int b = 0; b < BB; ++b) {
-      asm("mov.b64 {%0, %1}, %2;" : "=f"(acc[b][0]), "=f"(acc[b][1]) : "l"(acc2[b][0]));
-      asm("mov.b64 {%0, %1}, %2;" : "=f"(acc[b][2]), "=f"(acc[b][3]) : "l"(acc2[b][1]));
-    }
     // fold the 32/CQ lanes that share an output quad
 #pragma unroll
     for (int b = 0; b < BB; ++b)
@@ -349,13 +314,12 @@ lc3d_patch_kernel(const __grid_constant__ CUtensorMap tm_x, const float* __restr
 
 // ---------------------------------------------------------------------------------------
 // row kernel (batch >= 4, Cout = 16).  In lc3d_patch_kernel a lane owns ONE output quad and a slice of the patch
-// features: per float4 of weights it gets from shared memory (16 B) and per input value (4 B) it issues 2 * BB packed
-// FMAs, i.e. 4-6 bytes of shared-memory traffic per FFMA2 and lane.  The shared-memory crossbar delivers 128 B per clock
-// and SM, the FMA pipes take 128 lane-FFMA2 per clock: at batch 8 that kernel needs ~1300 crossbar cycles per position
-// against the 1180 cycles the position's 27.6 KB weight block takes to arrive from HBM (profiles/r02_ncu_full_lc3d_b8.txt:
-// shared-memory wavefronts 67 %, short-scoreboard stalls 3.6 per issue).
+// features: per float4 of weights it gets from shared memory (16 B) and per input value (4 B) it issues 4 * BB FMAs,
+// i.e. 2-3 bytes of shared-memory traffic per FMA and lane.  The shared-memory crossbar delivers 128 B per clock and SM,
+// the FMA pipes take 128 lane-FMAs per clock, so at batch 8 that kernel is bound by the crossbar, not by the weight
+// stream from HBM.
 // Here a lane owns patch ROWS j = lane, lane + 32, ... and ALL 16 output channels of BB batch items: a weight row
-// (64 B) and BB input values feed 8 * BB FFMA2 -- 1.25-1.5 B per FFMA2 and lane -- and the 16 * BB partial sums of the
+// (64 B) and BB input values feed 16 * BB FMAs -- 0.6-0.75 B per FMA and lane -- and the 16 * BB partial sums of the
 // 32 lanes are folded once per position with a reduce-scatter of shuffles (each step halves what a lane still holds).
 // Bank conflicts: rows are 64 B apart, so the lanes of a quarter-warp would hit two bank groups with the same chunk of
 // their rows; lane l therefore reads its row's four 16-byte chunks in the order q ^ m, m = (l >> 1) & 3, and accumulates
@@ -367,10 +331,7 @@ lc3d_patch_kernel(const __grid_constant__ CUtensorMap tm_x, const float* __restr
 // chunk of lane l ^ 2d: one shuffle per set and value sends every chunk to its owner.
 // Same ring, barriers and TMA patch load as lc3d_patch_kernel.  Summation order differs from the other kernels
 // (rows are summed lane-wise first): results agree to fp32 rounding, not bit for bit.
-// Measured on B200 at cfg 4, batch 8 (profiles/README.md): <4,2> (two warps x four items per position) 1.354-1.417 ms =
-// 0.74-0.77 of the HBM roofline, power-capped at 1695-1785 MHz (1.224 ms in a single launch under ncu); <8,1> 1.653 ms
-// (255 registers, 4-5 consumer warps); lc3d_patch_kernel<2,4> on the same box 1.814 ms.  Batch 4: <4,1> 1.323 ms vs
-// 1.232 ms for lc3d_patch_kernel<2,2>, which therefore keeps the passes of four.
+// Batch 4 keeps lc3d_patch_kernel<2,2>; batch 8 and more take <4,2> (two warps x four items per position).
 // ---------------------------------------------------------------------------------------
 template <int N>
 __device__ __forceinline__ void fold_upper(float* v, int mask) {      // v[0 .. N/2) += partner's v[N/2 .. N)
@@ -437,45 +398,28 @@ lc3d_rows_kernel(const __grid_constant__ CUtensorMap tm_x, const float* __restri
     const float4* wq2 = reinterpret_cast<const float4*>(base) + lane * 4 + (2 ^ m);
     const float4* wq3 = reinterpret_cast<const float4*>(base) + lane * 4 + (3 ^ m);
     const float* xp = reinterpret_cast<const float*>(base + patch_off) + (size_t)sub * BB * g.F + lane;
-    unsigned long long acc2[BB][8];                      // [slot][register set q, pair] = channels 4 * (q ^ m) + 2 * pair ..
+    float v[BB * 16];                                    // [slot][register set q][e] = channel 4 * (q ^ m) + e
 #pragma unroll
-    for (int b = 0; b < BB; ++b)
-#pragma unroll
-      for (int i = 0; i < 8; ++i) acc2[b][i] = 0ull;
+    for (int i = 0; i < BB * 16; ++i) v[i] = 0.f;
     if (k >= stages) mbar_wait(empty + slot, ph ^ 1u, 2000000 + k);      // parity aliasing guard (lc3d_patch_kernel)
     mbar_wait(full + slot, ph, k);
 #pragma unroll 2
     for (int c = 0; c < iters; ++c) {
       if (lane + (c << 5) < g.F) {                       // ragged last step: rows past F do not exist
         const float4 w0 = wq0[c * 128], w1 = wq1[c * 128], w2 = wq2[c * 128], w3 = wq3[c * 128];
-        unsigned long long wp[8];
-        asm("mov.b64 %0, {%1, %2};" : "=l"(wp[0]) : "f"(w0.x), "f"(w0.y));
-        asm("mov.b64 %0, {%1, %2};" : "=l"(wp[1]) : "f"(w0.z), "f"(w0.w));
-        asm("mov.b64 %0, {%1, %2};" : "=l"(wp[2]) : "f"(w1.x), "f"(w1.y));
-        asm("mov.b64 %0, {%1, %2};" : "=l"(wp[3]) : "f"(w1.z), "f"(w1.w));
-        asm("mov.b64 %0, {%1, %2};" : "=l"(wp[4]) : "f"(w2.x), "f"(w2.y));
-        asm("mov.b64 %0, {%1, %2};" : "=l"(wp[5]) : "f"(w2.z), "f"(w2.w));
-        asm("mov.b64 %0, {%1, %2};" : "=l"(wp[6]) : "f"(w3.x), "f"(w3.y));
-        asm("mov.b64 %0, {%1, %2};" : "=l"(wp[7]) : "f"(w3.z), "f"(w3.w));
+        const float w[16] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w,
+                             w2.x, w2.y, w2.z, w2.w, w3.x, w3.y, w3.z, w3.w};
 #pragma unroll
         for (int b = 0; b < BB; ++b) {
           const float xv = xp[xoff[b] + (c << 5)];
-          unsigned long long xx;
-          asm("mov.b64 %0, {%1, %1};" : "=l"(xx) : "f"(xv));
 #pragma unroll
-          for (int i = 0; i < 8; ++i) asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc2[b][i]) : "l"(xx), "l"(wp[i]));
+          for (int i = 0; i < 16; ++i) v[b * 16 + i] = fmaf(xv, w[i], v[b * 16 + i]);
         }
       }
     }
     __syncwarp();
     if (lane == 0) mbar_arrive(empty + slot);            // slot free: every lane has read its rows
     // ---- fold the 32 lanes' partial sums: v[slot][register set][channel in chunk]
-    float v[BB * 16];
-#pragma unroll
-    for (int b = 0; b < BB; ++b)
-#pragma unroll
-      for (int i = 0; i < 8; ++i)
-        asm("mov.b64 {%0, %1}, %2;" : "=f"(v[b * 16 + 2 * i]), "=f"(v[b * 16 + 2 * i + 1]) : "l"(acc2[b][i]));
     fold_upper<BB * 16>(v, 16);
     fold_upper<BB * 8>(v, 8);
     if (BB == 8) fold_upper<BB * 4>(v, 1);
@@ -580,7 +524,7 @@ lc3d_bwd_kernel(const float* __restrict__ x, const float* __restrict__ kernel, c
   }
 }
 
-template <int BB, int WPP, bool P2 = false>
+template <int BB, int WPP>
 static int launch_stream(const float* x, const float* kernel, const float* bias, float* out, const LcGeo& g,
                          int b_base, int cq_log2, cudaStream_t st) {
   const uint32_t blk_bytes = (uint32_t)g.F * g.Cout * sizeof(float);
@@ -590,7 +534,7 @@ static int launch_stream(const float* x, const float* kernel, const float* bias,
   if (stages < 2) return 1;                      // caller falls back to the generic kernel
   if (stages > kLcMaxStages) stages = kLcMaxStages;
   const size_t smem = (size_t)stages * blk_stride + (size_t)stages * 16 + (size_t)g.F * sizeof(int) + 16;
-  auto kern = lc3d_stream_kernel<BB, WPP, P2>;
+  auto kern = lc3d_stream_kernel<BB, WPP>;
   if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
     return check_launch("cudaFuncSetAttribute(lc3d_stream)");
   int grid = sm_count();
@@ -716,12 +660,10 @@ extern "C" int nrt_lc3d_fwd_f32(const float* x, const float* kernel, const float
     int cq_log2 = 0;
     while ((1 << cq_log2) < cq) ++cq_log2;
     int b = 0, rc = NRT_OK;
-    const char* pe = getenv("NRT_LC3D_FFMA2");
-    const bool p2 = !(pe && atoi(pe) == 0);
     const bool patch = env_int("NRT_LC3D_PATCH", 1) != 0;
     while (b < B && rc == NRT_OK) {              // batch items per pass = BB * WPP (weights streamed once per pass)
       const int left = B - b;
-      // one batch item: the TMA-patch kernel too (1.01 ms vs 1.16 ms for the register-gather kernel at cfg 4, B200)
+      // one batch item: the TMA-patch kernel too
       if (patch && left == 1 && env_int("NRT_LC3D_PATCH1", 1)) {
         const int prc = launch_patch<1, 1>(x, kernel, bias, out, g, b, cq_log2, st);
         if (prc <= 0) { rc = prc; b += 1; continue; }
@@ -743,10 +685,9 @@ extern "C" int nrt_lc3d_fwd_f32(const float* x, const float* kernel, const float
           if (prc <= 0) { rc = prc; b += 2; continue; }
         }
       }
-      // batch > 1 is FMA-issue bound: packed fp32x2 FMAs (NRT_LC3D_FFMA2=0 restores the scalar chain)
-      if (left >= 8) { rc = p2 ? launch_stream<4, 2, true>(x, kernel, bias, out, g, b, cq_log2, st) : launch_stream<4, 2>(x, kernel, bias, out, g, b, cq_log2, st); b += 8; }
-      else if (left >= 4) { rc = p2 ? launch_stream<2, 2, true>(x, kernel, bias, out, g, b, cq_log2, st) : launch_stream<2, 2>(x, kernel, bias, out, g, b, cq_log2, st); b += 4; }
-      else if (left >= 2) { rc = p2 ? launch_stream<2, 1, true>(x, kernel, bias, out, g, b, cq_log2, st) : launch_stream<2, 1>(x, kernel, bias, out, g, b, cq_log2, st); b += 2; }
+      if (left >= 8) { rc = launch_stream<4, 2>(x, kernel, bias, out, g, b, cq_log2, st); b += 8; }
+      else if (left >= 4) { rc = launch_stream<2, 2>(x, kernel, bias, out, g, b, cq_log2, st); b += 4; }
+      else if (left >= 2) { rc = launch_stream<2, 1>(x, kernel, bias, out, g, b, cq_log2, st); b += 2; }
       else { rc = launch_stream<1, 1>(x, kernel, bias, out, g, b, cq_log2, st); b += 1; }
     }
     if (rc <= 0) return rc;       // rc == 1: weight block does not fit the ring -> generic

@@ -1,5 +1,5 @@
 // nrt_metrics.cu -- Dice partial sums / finalize, hard-Dice label counts, argmax, and the
-// label-weighted categorical cross-entropy, for sm_100a.
+// label-weighted categorical cross-entropy, for sm_90a.
 //
 // All of these are pure HBM streams (8 B per (voxel,label), SURVEY.md 8d): coalesced
 // 128-bit loads that bypass L1, several independent loads in flight per thread, fixed
@@ -181,8 +181,8 @@ __global__ void dice_combine_serial_kernel(const float* __restrict__ partial, in
   }
 }
 
-// The same in two levels (3L <= blockDim): the serial kernel's 48 threads each walk all ~300 block partials, a 37 us
-// tail behind a 507 us streaming kernel (profiles/r02_launches_bench.csv).  Here slice s of blockDim / 3L slices sums
+// The same in two levels (3L <= blockDim): the serial kernel's 48 threads each walk all ~300 block partials, a long
+// serial tail behind the streaming kernel.  Here slice s of blockDim / 3L slices sums
 // blocks s, s + nslice, ... (consecutive threads read consecutive outputs: coalesced), then one thread per output adds
 // the slices in order.  fp64, fixed order.
 __global__ void dice_combine_kernel(const float* __restrict__ partial, int nblk, int L,
@@ -253,9 +253,8 @@ struct CceArgs {
 
 // Q = C/4 lanes per row (a power of two <= 32, compile time: the group shuffles unroll, no loop counters, no branches):
 // perfectly coalesced float4 streams; U rows per thread and pass, i.e. U independent pairs of streaming loads in flight
-// per thread.  The first version (profiles/r02_ncu_full_cce.txt) took q at run time and ran one load pair per thread:
-// 8.6 long-scoreboard stall cycles per issue at 74 % issue-active with half of its instructions on the ALU pipe, 0.84 of
-// the HBM roofline; two rows per thread 0.90, four 1.00 (profiles/r02_ncu_full_cce_u4.txt).
+// per thread (a run-time q with one load pair per thread stalls on long-scoreboard waits and spends half of its
+// instructions on the ALU pipe).
 template <int Q>
 __device__ __forceinline__ float group_sum_c(float v) {
 #pragma unroll

@@ -12,7 +12,7 @@
 // (relative error 2^-21 per product, far inside the 1e-5 parity tolerance), accumulators
 // flushed into fp32 registers every 128 voxels so tensor-core accumulation rounding cannot
 // build up, block partials combined in fp64 in a fixed order (deterministic results).
-// The output tile is only nb x nb (16..32), so tcgen05's 64/128-row tiles would idle 75 % of
+// The output tile is only nb x nb (16..32), so wgmma's 64-row warpgroup tiles would idle most of
 // the array; the warp-level mma shape fits the problem.  With soft quantisation the kernel is
 // bound by issue slots / MUFU (32 exponentials per voxel pair), not by HBM; with precomputed
 // probability maps (segs) it streams 8*nb bytes per voxel and is HBM-bound.
@@ -26,7 +26,7 @@ namespace {
 
 constexpr int kMiThreads = 256;
 constexpr int kMiWarps = kMiThreads / 32;
-constexpr int kMiMaxBlocks = 592;           // 4 CTAs per SM x 148
+constexpr int kMiMaxBlocks = 592;           // 4 CTAs per SM on up to 148 SMs (sizes the workspace)
 constexpr int kMiMaxBins = 64;
 
 struct MiOperand {
@@ -559,8 +559,8 @@ __global__ void soft_quantize_kernel(const float* x, int64_t n, const float* cen
 template <int MT, int NT, int SPCQ, int SPCM>
 void launch_mma(const MiArgs& a, dim3 grid, cudaStream_t st, int variant) {
   if (a.x.quant && a.y.quant) {
-    // 2 CTAs per SM measured best (1.02 ms vs 1.18 ms at 3 CTAs per SM for 8 volume pairs: the MUFU and
-    // tensor pipes are the limit, more resident warps only add contention).  NRT_MI_VARIANT (dev switch):
+    // 2 CTAs per SM: the MUFU and tensor pipes are the limit, more resident warps only add contention.
+    // NRT_MI_VARIANT (dev switch):
     // 1 = 2 steps per chunk at 3 CTAs per SM, 2 = 4 steps at 3 CTAs per SM
     if (variant == 1) mi_hist_mma_kernel<MT, NT, true, true, 2, 3><<<grid, kMiThreads, 0, st>>>(a);
     else if (variant == 2) mi_hist_mma_kernel<MT, NT, true, true, SPCQ, 3><<<grid, kMiThreads, 0, st>>>(a);

@@ -29,21 +29,11 @@ struct MarchGeo {
   int B, nchunk, nseg, seg_len; // channel chunks of CCH, z segments per column and their length
   int64_t src_batch_stride, out_vox;
   int64_t flow_bstride, out_bstride;   // elements between batch items of flow / out
-  f32x2 negzero2, one2;         // (-0,-0), (1,1): identity operands of the packed arithmetic
 };
-
-// -DNRT_MARCH_PACKED=1: quads (CPL == 4) interpolated with packed fp32x2 arithmetic (64 FFMA2 instead of 64 FMUL + 56
-// FADD per thread and plane; same bits).  Measured equal on B200 (C = 16: 0.511 / 0.469 ms i.i.d. / smooth vs 0.505-0.509 /
-// 0.463 scalar): the kernel waits on shared-memory wavefronts and plane arrivals, not on issue slots.  Off by default.
-#ifndef NRT_MARCH_PACKED
-#define NRT_MARCH_PACKED 0
-#endif
-constexpr bool kMarchPacked = NRT_MARCH_PACKED != 0;
 
 // CCH = channels staged per voxel (a chunk of the volume's C); VEC: lanes own 4-channel quads, else all CCH channels.
 // QPT = quads per thread (VEC only): the per-voxel corner setup (~60 instructions) and the 8 corner weights are
-// shared by the QPT quads a thread owns -- with one quad per thread they are 2/3 of all instructions
-// (profiles/r02_ncu_march16.txt: 227 per voxel-quad, issue-bound at 76 %).
+// shared by the QPT quads a thread owns -- with one quad per thread they are 2/3 of all instructions.
 // G = output planes in flight per CTA (plane groups of NW / G warps each, see the kernel): the ring then holds the
 // windows of G consecutive output planes plus AHEAD planes of prefetch.
 template <int CCH, int TY_, int TX_, int HALO_, int AHEAD_, int QPT_ = 1, int G_ = 1>
@@ -205,26 +195,12 @@ warp3d_march_kernel(const __grid_constant__ CUtensorMap tm_vol, const __grid_con
           lds_channels<CPL>(p0 + qo + dy, v[2]);      lds_channels<CPL>(p0 + qo + dy + dx, v[3]);
           lds_channels<CPL>(p1 + qo, v[4]);           lds_channels<CPL>(p1 + qo + dx, v[5]);
           lds_channels<CPL>(p1 + qo + dy, v[6]);      lds_channels<CPL>(p1 + qo + dy + dx, v[7]);
-          if (CPL == 4 && kMarchPacked) {
-            // packed: the channel pairs (0,1) and (2,3) of a corner are the two halves of the LDS.128 result, the
-            // corner weight is the broadcast operand; products and sums rounded separately as in the scalar chain
-            f32x2 r01 = 0ull, r23 = 0ull;                          // (+0, +0): 0 + k0 * v0 like the scalar chain
 #pragma unroll
-            for (int n = 0; n < 8; ++n) {
-              const f32x2 kk = pack2(k[n], k[n]);
-              r01 = fma2(fma2(kk, pack2(v[n][0], v[n][1 % CPL]), w.negzero2), w.one2, r01);
-              r23 = fma2(fma2(kk, pack2(v[n][2 % CPL], v[n][3 % CPL]), w.negzero2), w.one2, r23);
-            }
-            unpack2(r01, res[qi][0], res[qi][1 % CPL]);
-            unpack2(r23, res[qi][2 % CPL], res[qi][3 % CPL]);
-          } else {
+          for (int c = 0; c < CPL; ++c) {
+            float r = __fadd_rn(0.f, __fmul_rn(k[0], v[0][c]));
 #pragma unroll
-            for (int c = 0; c < CPL; ++c) {
-              float r = __fadd_rn(0.f, __fmul_rn(k[0], v[0][c]));
-#pragma unroll
-              for (int n = 1; n < 8; ++n) r = __fadd_rn(r, __fmul_rn(k[n], v[n][c]));
-              res[qi][c] = r;
-            }
+            for (int n = 1; n < 8; ++n) r = __fadd_rn(r, __fmul_rn(k[n], v[n][c]));
+            res[qi][c] = r;
           }
         }
       } else {
@@ -348,13 +324,6 @@ int warp3d_march(const float* vol, const float* flow, float* out, int B, const i
   mg.g.has_fill = has_fill; mg.g.fill = fill; mg.g.err = err_flag;
   mg.out_z0 = out_z0; mg.out_n0 = out_n0; mg.B = B;
   mg.nchunk = mg.nseg = mg.seg_len = 1;
-  {
-    const float nzf = -0.0f, onef = 1.0f;
-    uint32_t nzb, oneb;
-    memcpy(&nzb, &nzf, 4); memcpy(&oneb, &onef, 4);
-    mg.negzero2 = ((f32x2)nzb << 32) | nzb;
-    mg.one2 = ((f32x2)oneb << 32) | oneb;
-  }
   mg.out_vox = (int64_t)out_n0 * H * W;
   mg.src_batch_stride = vbs ? vbs : (int64_t)src_n0 * H * W * C;
   mg.flow_bstride = fbs ? fbs : mg.out_vox * 3;
@@ -362,8 +331,8 @@ int warp3d_march(const float* vol, const float* flow, float* out, int B, const i
   if ((mg.src_batch_stride | mg.flow_bstride | mg.out_bstride) & 3) return NRT_OK;   // TMA strides: multiples of 16 bytes
   int rc = 1;
   const int nw16 = env_int("NRT_MARCH_NW", 16);
-  // quads per thread: 2 by default for 8 / 16-channel chunks (measured, profiles/r02_sweep_visit2.txt: smooth flows
-  // 0.63 vs 0.59 of the roofline at C = 16, i.i.d. flows 0.55 vs 0.56 -- those are bank-conflict bound either way)
+  // quads per thread: 2 by default for 8 / 16-channel chunks (the corner setup is shared by two quads; i.i.d. flows
+  // are bank-conflict bound either way)
   const int qpt = env_int("NRT_MARCH_QPT", 2);
 #define NRT_MARCH(cch, ty, tx, ahead, nw)                                                                      \
   rc = method == NRT_LINEAR ? launch_march<cch, ty, tx, 3, ahead, nw, NRT_LINEAR>(vol, flow, out, mg, st)      \
@@ -371,9 +340,8 @@ int warp3d_march(const float* vol, const float* flow, float* out, int B, const i
 #define NRT_MARCH_Q(cch, ty, tx, ahead, nw, qq)                                                                \
   rc = method == NRT_LINEAR ? launch_march<cch, ty, tx, 3, ahead, nw, NRT_LINEAR, qq>(vol, flow, out, mg, st)  \
                             : launch_march<cch, ty, tx, 3, ahead, nw, NRT_NEAREST, qq>(vol, flow, out, mg, st)
-  // (two output planes in flight per CTA -- template parameter G = 2: 16 consumer warps with two quads per thread, ring
-  // 7 + 1 + 2 -- measured the same as one, C = 16 i.i.d. 0.584 vs 0.573, smooth 0.627 vs 0.633: the kernel is not short
-  // of warps.  Not instantiated.)
+  // (two output planes in flight per CTA -- template parameter G = 2 -- is not instantiated: the kernel is not short
+  // of warps.)
   if (C % 16 == 0) {
     // QPT 2 / 4: a thread owns 8 / 16 channels of its voxel and shares the corner setup between them
     if (qpt == 4) NRT_MARCH_Q(16, 8, 16, 3, 4, 4);

@@ -1,6 +1,6 @@
 """
 neurite_b200.layers -- drop-ins for the hot-path layers of neurite.layers
-(/root/reference/neurite/tf/layers.py) as torch.nn.Modules on channels-last CUDA tensors.
+(adalca/neurite: neurite/tf/layers.py) as torch.nn.Modules on channels-last CUDA tensors.
 
     Resize / Zoom           layers.py:91-185
     SpatialTransformer      voxelmorph.layers.SpatialTransformer (call sites models.py:806, 1157)

@@ -1,5 +1,5 @@
 """
-neurite_b200.losses -- the loss shells of neurite.losses (/root/reference/neurite/tf/losses.py:46-205):
+neurite_b200.losses -- the loss shells of neurite.losses (adalca/neurite: neurite/tf/losses.py:46-205):
 `loss = -dice` ([batch, nb_labels]), `mean_loss = -mean_dice` (scalar), and
 CategoricalCrossentropy.loss = cce.  Bound methods are `(y_true, y_pred) -> Tensor` callables,
 the protocol the reference hands to model.compile(loss=...) and callbacks.PredictMetrics.

@@ -1,6 +1,6 @@
 """
 neurite_b200.metrics -- drop-ins for Dice / SoftDice / HardDice / CategoricalCrossentropy of
-neurite.metrics (/root/reference/neurite/tf/metrics.py:339-650) on torch CUDA tensors.
+neurite.metrics (adalca/neurite: neurite/tf/metrics.py:339-650) on torch CUDA tensors.
 
 Same constructor arguments, defaults, assertions and method names (`dice`, `mean_dice`,
 `loss`, `cce`, `__call__`).  tf.debugging asserts become `InvalidArgumentError`

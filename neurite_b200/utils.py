@@ -1,6 +1,6 @@
 """
 neurite_b200.utils -- drop-in for the interpolation part of neurite.utils
-(/root/reference/neurite/tf/utils/utils.py), on torch CUDA tensors, channels-last.
+(adalca/neurite: neurite/tf/utils/utils.py), on torch CUDA tensors, channels-last.
 
     interpn(vol, loc, interp_method='linear', fill_value=None)     utils.py:73-220
     resize(vol, zoom_factor, interp_method='linear') / zoom        utils.py:223-265

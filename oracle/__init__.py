@@ -5,7 +5,7 @@ This package is the *checker*, never the product.  Only ``tests/``,
 ``__graft_entry__.smoke()`` and ``bench.py``'s ``cpu_baseline`` / ``--impl reference``
 legs may import it.  ``neurite_b200`` (the product) never imports, links or calls it.
 
-What it restates (all citations are into /root/reference, adalca/neurite @ 7c4b05e):
+What it restates (all citations are into adalca/neurite @ 7c4b05e):
 
   interp.py   neurite/tf/utils/utils.py:73-220   interpn (linear / nearest / fill_value)
               neurite/tf/utils/utils.py:223-265  resize / zoom
@@ -30,7 +30,7 @@ The reference ships no tests, fixtures or golden vectors for this path (SURVEY.m
 and TensorFlow cannot be imported in this image.  Parity is pinned as follows:
 
   * tests/golden/*.npz were produced by executing the REFERENCE'S OWN python source
-    (imported from /root/reference, unmodified) on top of ``tools/tfshim`` -- a numpy
+    (imported from a reference checkout, unmodified) on top of ``tools/tfshim`` -- a numpy
     implementation of the ~60 TensorFlow/Keras ops those functions call.  The generating
     script is tools/gen_golden.py.  The algorithm (clip/cast order, corner order,
     weight products, fill mask, Dice sums, patch ordering) is therefore the
@@ -41,7 +41,7 @@ and TensorFlow cannot be imported in this image.  Parity is pinned as follows:
     torch grid_sample(border, align_corners=True), F.conv3d with position-shared weights,
     scipy.ndimage.correlate1d and F.conv3d for the separable convolutions, the plug-in
     entropy / hard-histogram limits for MutualInformation.
-  * third-party arithmetic that is NOT in /root/reference (voxelmorph
+  * third-party arithmetic that is NOT in the reference (voxelmorph
     SpatialTransformer, Keras CategoricalCrossentropy, tf.linspace, tf.nn.convolution) is
     restated from its published definition: for those pieces parity is UNPINNED by the
     reference repo itself and says so in DESIGN.md.

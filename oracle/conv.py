@@ -2,7 +2,7 @@
 numpy restatement of gaussian_kernel / separable_conv / GaussianBlur / subsample_axis.
 TEST INFRASTRUCTURE (see oracle/__init__.py).
 
-Follows /root/reference/neurite/tf:
+Follows adalca/neurite: neurite/tf:
     utils/utils.py:581-662   gaussian_kernel
     utils/utils.py:665-751   separable_conv   (tf.nn.convolution: third party, TF unpinned --
                              cross-correlation, 'SAME' = zero padding with the extra element at

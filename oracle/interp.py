@@ -3,7 +3,7 @@ numpy fp32 restatement of the reference's N-D gridded interpolation.  TEST INFRA
 (see oracle/__init__.py) -- op-for-op, so every intermediate is rounded to fp32 exactly
 where TensorFlow would round it (each TF op materialises an fp32 tensor; nothing is fused).
 
-Follows /root/reference/neurite/tf/utils/utils.py:
+Follows adalca/neurite: neurite/tf/utils/utils.py:
     interpn      :73-220
     resize/zoom  :223-265
     ndgrid/meshgrid/volshape_to_ndgrid/volshape_to_meshgrid  :333-476

@@ -2,7 +2,7 @@
 numpy fp32 restatement of LocallyConnected3D, implementation 1.  TEST INFRASTRUCTURE
 (see oracle/__init__.py).
 
-Follows /root/reference/neurite/tf/layers.py:
+Follows adalca/neurite: neurite/tf/layers.py:
     build (shapes)            :951-1047
     call (bias, activation)   :1072-1102
     local_conv (impl 1)       :1126-1197

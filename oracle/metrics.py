@@ -2,7 +2,7 @@
 numpy fp32 restatement of Dice and the label-weighted categorical cross-entropy.
 TEST INFRASTRUCTURE (see oracle/__init__.py).
 
-Follows /root/reference/neurite/tf:
+Follows adalca/neurite: neurite/tf:
     metrics.py:352-413   Dice.__init__ (argument checks)
     metrics.py:415-482   Dice.dice
     metrics.py:484-510   Dice.mean_dice

@@ -2,7 +2,7 @@
 numpy fp32 restatement of soft_quantize and MutualInformation.
 TEST INFRASTRUCTURE (see oracle/__init__.py).
 
-Follows /root/reference/neurite/tf:
+Follows adalca/neurite: neurite/tf:
     utils/utils.py:1099-1172  soft_quantize (bin centres default to tf.linspace(min x, max x, nb))
     metrics.py:69-114         MutualInformation.__init__ (alpha = 1 / (2 sigma^2), fp32)
     metrics.py:116-138        volumes          metrics.py:140-152  segs

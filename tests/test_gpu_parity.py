@@ -1,5 +1,5 @@
 """
-GPU parity tests (run on the B200 box: `pytest -m gpu`).  Everything goes through the public
+GPU parity tests (run on an H100: `pytest -m gpu`).  Everything goes through the public
 python API -> ctypes -> the C ABI of libneurite_b200.so.  Checked against
   * tests/golden/*.npz   (outputs of the reference's own source, see tools/gen_golden.py)
   * the numpy oracle      (oracle/, same seeded inputs, incl. BASELINE.json's full 160x192x224)
@@ -351,12 +351,11 @@ def test_lc3d_golden(ne, monkeypatch, name, generic):
     np.testing.assert_allclose(out, g['out'], rtol=1e-5, atol=2e-5)
 
 
-@pytest.mark.parametrize('ffma2,patch', [('1', '1'), ('1', '0'), ('0', '0')])
-def test_lc3d_vs_oracle_batches_activations_and_sharding(ne, monkeypatch, ffma2, patch):
-    """batch 11 = passes of 8 + 2 + 1 items: the TMA-patch kernel (batch > 1), the register-gather kernel with
-    packed (fp32x2) and with scalar accumulation chains are bit-identical, all within 1e-5 of the oracle."""
+@pytest.mark.parametrize('patch', ['1', '0'])
+def test_lc3d_vs_oracle_batches_activations_and_sharding(ne, monkeypatch, patch):
+    """batch 11 = passes of 8 + 2 + 1 items: the TMA-patch kernel (batch > 1) and the register-gather kernel are
+    bit-identical, all within 1e-5 of the oracle."""
     from neurite_b200.layers import local_conv3d
-    monkeypatch.setenv('NRT_LC3D_FFMA2', ffma2)
     monkeypatch.setenv('NRT_LC3D_PATCH', patch)
     rng = np.random.default_rng(13)
     x = rng.standard_normal((11, 8, 9, 10, 16)).astype(F32)
@@ -367,23 +366,20 @@ def test_lc3d_vs_oracle_batches_activations_and_sharding(ne, monkeypatch, ffma2,
         ref = olc3d.locally_connected_3d(x, kernel, bias, (3, 3, 3), activation=act, literal=False)
         out = local_conv3d(dev(x), dev(kernel), dev(bias), (3, 3, 3), (1, 1, 1), O, activation=act).cpu().numpy()
         np.testing.assert_allclose(out, ref, rtol=1e-5, atol=2e-5)
-    if ffma2 == '1':
-        # (the quad-per-lane kernels share one summation order; the row kernels are compared in their own test)
-        monkeypatch.setenv('NRT_LC3D_ROWS', '0')
-        out = local_conv3d(dev(x), dev(kernel), dev(bias), (3, 3, 3), (1, 1, 1), O, activation='sigmoid').cpu().numpy()
-        monkeypatch.setenv('NRT_LC3D_FFMA2', '0')
-        monkeypatch.setenv('NRT_LC3D_PATCH', '0')
-        scalar = local_conv3d(dev(x), dev(kernel), dev(bias), (3, 3, 3), (1, 1, 1), O, activation='sigmoid').cpu().numpy()
-        np.testing.assert_array_equal(out, scalar)
-        monkeypatch.setenv('NRT_LC3D_FFMA2', '1')
-        monkeypatch.setenv('NRT_LC3D_PATCH', patch)
-        # strides > 1 and a ragged weight block (F * Cout / 4 not a multiple of 32): patch origin = position * stride
-        xs = rng.standard_normal((4, 9, 8, 11, 4)).astype(F32)
-        Os = (4, 3, 5)
-        ks = (rng.standard_normal((int(np.prod(Os)), 2 * 3 * 2 * 4, 4)) * 0.1).astype(F32)
-        refs = olc3d.locally_connected_3d(xs, ks, None, (2, 3, 2), strides=(2, 2, 2), literal=False)
-        outs = local_conv3d(dev(xs), dev(ks), None, (2, 3, 2), (2, 2, 2), Os).cpu().numpy()
-        np.testing.assert_allclose(outs, refs, rtol=1e-5, atol=2e-5)
+    # (the quad-per-lane kernels share one summation order; the row kernels are compared in their own test)
+    monkeypatch.setenv('NRT_LC3D_ROWS', '0')
+    out = local_conv3d(dev(x), dev(kernel), dev(bias), (3, 3, 3), (1, 1, 1), O, activation='sigmoid').cpu().numpy()
+    monkeypatch.setenv('NRT_LC3D_PATCH', '0')
+    gather = local_conv3d(dev(x), dev(kernel), dev(bias), (3, 3, 3), (1, 1, 1), O, activation='sigmoid').cpu().numpy()
+    np.testing.assert_array_equal(out, gather)
+    monkeypatch.setenv('NRT_LC3D_PATCH', patch)
+    # strides > 1 and a ragged weight block (F * Cout / 4 not a multiple of 32): patch origin = position * stride
+    xs = rng.standard_normal((4, 9, 8, 11, 4)).astype(F32)
+    Os = (4, 3, 5)
+    ks = (rng.standard_normal((int(np.prod(Os)), 2 * 3 * 2 * 4, 4)) * 0.1).astype(F32)
+    refs = olc3d.locally_connected_3d(xs, ks, None, (2, 3, 2), strides=(2, 2, 2), literal=False)
+    outs = local_conv3d(dev(xs), dev(ks), None, (2, 3, 2), (2, 2, 2), Os).cpu().numpy()
+    np.testing.assert_allclose(outs, refs, rtol=1e-5, atol=2e-5)
     # position sharding: two ranks each own half of the positions AND of the weights
     ref = olc3d.locally_connected_3d(x, kernel, bias, (3, 3, 3), literal=False).reshape(11, -1, 16)
     P = kernel.shape[0]
@@ -430,7 +426,7 @@ def test_lc3d_row_kernel_vs_oracle(ne, monkeypatch, rows):
 
 @pytest.mark.parametrize('rows', ['1', '0'])
 def test_lc3d_batch8_shared_weights_equal_conv3d(ne, monkeypatch, rows):
-    """cfg 4 geometry, batch 8, many positions per CTA (22^3 positions over 148 CTAs: every ring slot is reused many
+    """cfg 4 geometry, batch 8, many positions per CTA (22^3 positions over 132 CTAs: every ring slot is reused many
     times): with position-shared weights the layer must equal a plain conv3d"""
     monkeypatch.setenv('NRT_LC3D_ROWS', rows)
     rng = np.random.default_rng(19)

@@ -2,11 +2,11 @@
 """
 tools/gen_golden.py -- generate tests/golden/*.npz by EXECUTING THE REFERENCE'S OWN SOURCE.
 
-    python tools/gen_golden.py            # needs /root/reference (this container only)
+    python tools/gen_golden.py REFERENCE_ROOT     # a checkout of adalca/neurite @ 7c4b05e
 
 The reference (adalca/neurite @ 7c4b05e) is pure Python on TensorFlow, and TensorFlow is
 not installable here.  tools/tfshim.py supplies a numpy implementation of the leaf TF ops;
-this script imports `neurite` from /root/reference unmodified and calls
+this script imports `neurite` from REFERENCE_ROOT unmodified and calls
 
     neurite.utils.interpn / resize / volshape_to_meshgrid           (tf/utils/utils.py)
     neurite.layers.Resize, neurite.layers.LocallyConnected3D         (tf/layers.py)
@@ -15,11 +15,11 @@ this script imports `neurite` from /root/reference unmodified and calls
 
 on seeded inputs, storing inputs + outputs.  Each fixture's `provenance` field says which
 reference symbol produced it.  Two fixtures are *compositions by contract* because their
-arithmetic lives in packages absent from /root/reference (SURVEY.md 8c): `st_*`
+arithmetic lives in packages absent from the reference (SURVEY.md 8c): `st_*`
 (voxelmorph SpatialTransformer = reference meshgrid + flow -> reference interpn) and the
 Keras CCE formula inside tfshim.  They are labelled provenance='contract'.
 
-The fixtures travel to the GPU box (tests never read /root/reference at run time).
+The fixtures are committed: tests never read the reference at run time.
 """
 import os
 import sys
@@ -31,7 +31,9 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
 import tfshim  # noqa: E402
 
-ne = tfshim.install('/root/reference')
+if len(sys.argv) != 2:
+    raise SystemExit('usage: python tools/gen_golden.py REFERENCE_ROOT')
+ne = tfshim.install(sys.argv[1])
 T = tfshim.Tensor
 OUT = os.path.join(os.path.dirname(HERE), 'tests', 'golden')
 os.makedirs(OUT, exist_ok=True)

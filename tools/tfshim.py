@@ -1,10 +1,10 @@
 """
 tools/tfshim.py -- a numpy stand-in for the TensorFlow/Keras ops that the reference's hot
-path calls, so that the reference's OWN python source (imported unmodified from
-/root/reference) can be executed in this image, where TensorFlow is not installed.
+path calls, so that the reference's OWN python source (imported unmodified from a
+checkout of adalca/neurite) can be executed where TensorFlow is not installed.
 
 Used only by tools/gen_golden.py to produce tests/golden/*.npz.  It is not part of the
-product, not part of the oracle, and never runs on the GPU box.
+product, not part of the oracle, and never runs on the GPU.
 
 Design
   * `Tensor` is an immutable wrapper around an np.ndarray (TF tensors are immutable: the
@@ -530,7 +530,7 @@ def _install_tf():
     return tf
 
 
-def install(reference_root='/root/reference'):
+def install(reference_root):
     """Install the shim and return the imported reference package `neurite`."""
     if 'neurite' in sys.modules:
         return sys.modules['neurite']
@@ -538,6 +538,6 @@ def install(reference_root='/root/reference'):
     sys.meta_path.insert(0, _Finder())
     if reference_root not in sys.path:
         sys.path.insert(0, reference_root)
-    sys.dont_write_bytecode = True            # /root/reference is read-only
+    sys.dont_write_bytecode = True            # the reference checkout may be read-only
     import neurite
     return neurite
