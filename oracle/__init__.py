@@ -19,6 +19,9 @@ What it restates (all citations are into adalca/neurite @ 7c4b05e):
   mi.py       neurite/tf/metrics.py:41-336       MutualInformation (volumes / segs / volume_seg /
               channelwise / maps), neurite/tf/utils/utils.py:1099-1172 soft_quantize;
               plus a float64 torch restatement of the same graph as the GRADIENT oracle
+  grad.py     differentiable torch restatements of interpn / warp / resize / VecInt / Dice / CCE /
+              LocallyConnected3D (the GRADIENT oracle of the other ops) and the per-element
+              gradient error bound the GPU gradient tests use
   conv.py     neurite/tf/utils/utils.py:581-751  gaussian_kernel / separable_conv,
               neurite/tf/layers.py:251-364 GaussianBlur, utils.py:754-826 subsample_axis
   c/          the same arithmetic as fused C99 + OpenMP loops (fast enough for full-size

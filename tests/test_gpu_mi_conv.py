@@ -340,3 +340,20 @@ def test_mi_segs_and_volume_seg_gradient(ne):
         (omi.torch_volume_seg(vt, st, nb_bins=L, alpha=float(m.soft_bin_alpha)) * w.double()).sum().backward()
         _grad_close(v.grad, vt.grad)
         _grad_close(s.grad, st.grad)
+
+
+@pytest.mark.parametrize('nb', [16, 32])
+def test_mi_volumes_gradient_many_ctas(ne, nb):
+    """V = 2^17 + 13 voxels per item: the centre-gradient partials of many CTAs of mi_bwd_voxel_kernel are combined
+    by mi_bwd_combine_kernel."""
+    rng = np.random.default_rng(200 + nb)
+    x = rng.uniform(0, 1, (2, 2 ** 17 + 13, 1)).astype(F32)
+    y = np.clip(0.5 * x ** 2 + 0.3 + 0.1 * rng.standard_normal(x.shape), 0, 1).astype(F32)
+    w = rng.standard_normal(2)
+    xg, yg = dev(x).requires_grad_(True), dev(y).requires_grad_(True)
+    m = ne.metrics.MutualInformation(nb_bins=nb)
+    (m.volumes(xg, yg) * dev(w.astype(F32))).sum().backward()
+    xt, yt = torch.from_numpy(x).double().requires_grad_(True), torch.from_numpy(y).double().requires_grad_(True)
+    (omi.torch_channelwise(xt, yt, nb_bins=nb, alpha=float(m.soft_bin_alpha)) * torch.from_numpy(w)[:, None]).sum().backward()
+    _grad_close(xg.grad, xt.grad)
+    _grad_close(yg.grad, yt.grad)
