@@ -22,6 +22,9 @@ What it restates (all citations are into adalca/neurite @ 7c4b05e):
   grad.py     differentiable torch restatements of interpn / warp / resize / VecInt / Dice / CCE /
               LocallyConnected3D (the GRADIENT oracle of the other ops) and the per-element
               gradient error bound the GPU gradient tests use
+  forward.py  float64 forward references (Dice with normalize, hard-Dice counts, separable
+              convolution, MI joint histograms and bin centres) and the per-element bound of each
+              forward kernel, its depth derived from the launch geometry
   conv.py     neurite/tf/utils/utils.py:581-751  gaussian_kernel / separable_conv,
               neurite/tf/layers.py:251-364 GaussianBlur, utils.py:754-826 subsample_axis
   c/          the same arithmetic as fused C99 + OpenMP loops (fast enough for full-size

@@ -33,15 +33,19 @@ from .interp import tf_linspace_f32
 U = 2.0 ** -24
 
 
-def grad_close(got, ref, scale, k, c=4.0, what='gradient'):
-    """Assert |got - ref| <= c * k * 2^-24 * scale element by element (k: scalar or per element)."""
+def grad_close(got, ref, scale, k, c=4.0, what='gradient', approx=0.):
+    """Assert |got - ref| <= c * k * 2^-24 * scale + approx element by element (k, approx: scalar or per element).
+    approx is the documented error of an approximate hardware function (oracle/forward.py names each one); it is
+    0 for every gradient."""
     got = got.detach().to(torch.float64)
     ref = ref.detach().to(device=got.device, dtype=torch.float64)
     scale = torch.as_tensor(scale, dtype=torch.float64, device=got.device)
     k = torch.as_tensor(k, dtype=torch.float64, device=got.device)
+    approx = torch.as_tensor(approx, dtype=torch.float64, device=got.device)
     assert c <= 4
+    assert bool((approx >= 0).all())
     assert got.shape == ref.shape, '%s: shape %s vs reference %s' % (what, tuple(got.shape), tuple(ref.shape))
-    tol = c * k * U * scale
+    tol = c * k * U * scale + approx
     err = (got - ref).abs()
     bad = ~(err <= tol)
     if bool(bad.any()):
@@ -51,7 +55,8 @@ def grad_close(got, ref, scale, k, c=4.0, what='gradient'):
         idx = lambda n: tuple(int(v) for v in np.unravel_index(n, tuple(got.shape)))   # noqa: E731
         tb = lambda t, n: float(torch.broadcast_to(t, got.shape).reshape(-1)[n])         # noqa: E731
         raise AssertionError(
-            '%s: %d of %d elements outside c*k*2^-24*scale; first at %s: got %.9g ref %.9g tol %.3g (scale %.3g k %g); '
+            '%s: %d of %d elements outside c*k*2^-24*scale + approx; first at %s: got %.9g ref %.9g tol %.3g '
+            '(scale %.3g k %g); '
             'worst at %s: got %.9g ref %.9g tol %.3g'
             % (what, int(bad.sum()), bad.numel(), idx(i), float(got.reshape(-1)[i]), float(ref.reshape(-1)[i]),
                tb(tol, i), tb(scale, i), tb(k, i), idx(j), float(got.reshape(-1)[j]), float(ref.reshape(-1)[j]),
