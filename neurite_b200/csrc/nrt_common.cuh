@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+#include <stdlib.h>
 #include <stdarg.h>
 
 #include "../../include/neurite_b200.h"
@@ -26,6 +27,12 @@ int sm_count();
 // tiled backward of the D=3, C=1 warp (defined in nrt_interp.cu next to the forward tile kernel)
 int warp3d_bwd_tile(const float* vol, const float* flow, const float* gout, float* gvol, float* gflow, int B,
                     const int32_t* shape, int method, int has_fill, cudaStream_t st, bool* used);
+
+// the only reader of the NRT_* test / comparison switches (README.md): unset or empty gives dflt
+inline int env_int(const char* name, int dflt) {
+  const char* s = getenv(name);
+  return (s && *s) ? atoi(s) : dflt;
+}
 
 inline int64_t imin64(int64_t a, int64_t b) { return a < b ? a : b; }
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }

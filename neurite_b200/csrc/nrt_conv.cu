@@ -9,7 +9,7 @@
 // A tensor [B, *space, C] seen from axis a is [outer, L, inner] with inner = prod(space[a+1:]) * C
 // contiguous.  One pass reads and writes every element once (8 B per element is the roofline
 // of a pass); the taps come out of a shared-memory tile:
-//   * inner >= 32 ("column" pass): 128 (float4) or 32 inner elements x 32/64 outputs per CTA, every
+//   * inner >= 32 ("column" pass): 128 (float4) or 32 inner elements x 64 outputs per CTA, every
 //     thread slides a register window of outputs down the tile (8 shared loads per 32-64 FMAs);
 //   * inner <  32 ("row" pass, e.g. the last axis of a single-channel volume): a flat 2048-output
 //     segment + halo per CTA, row ends handled per tap;
@@ -86,14 +86,12 @@ __global__ void __launch_bounds__(256) sepconv_col_kernel(const ConvArgs a, int 
 }
 
 
-// float4 variant of the column pass: 128 inner elements x TL outputs per CTA, so every row of the
+// float4 variant of the column pass: 128 inner elements x kColTL outputs per CTA, so every row of the
 // tile is one 512-byte burst (the 32-wide tile reads 128-byte pieces 170 KB apart).  Needs
-// inner % 4 == 0 and 16-byte aligned tensors.  block (32, 8); thread = 4 inner x RL outputs.
-template <int TL>
+// inner % 4 == 0 and 16-byte aligned tensors.  block (32, 8); thread = 4 inner x kColRL outputs.
 __global__ void __launch_bounds__(256) sepconv_col4_kernel(const ConvArgs a, int Kp, int i_tiles, int l_tiles) {
-  constexpr int RL = TL / 8;
   extern __shared__ __align__(16) float smem[];
-  const int rows = TL + Kp - 1;
+  const int rows = kColTL + Kp - 1;
   float4* sm = reinterpret_cast<float4*>(smem);        // [rows][32] float4
   float* ks = smem + rows * 128;                       // [Kp], zero padded
   const int tx = threadIdx.x, ty = threadIdx.y, tid = ty * 32 + tx;
@@ -104,7 +102,7 @@ __global__ void __launch_bounds__(256) sepconv_col4_kernel(const ConvArgs a, int
   const int lt = (int)(blk % l_tiles);
   const int64_t o = blk / l_tiles;
   const int64_t i = (int64_t)it * 128 + tx * 4;
-  const int64_t l0 = (int64_t)lt * TL;
+  const int64_t l0 = (int64_t)lt * kColTL;
   const bool iok = i < a.inner;                        // inner % 4 == 0: a float4 is all in or all out
 
   for (int j = tid; j < Kp; j += 256) ks[j] = j < a.K ? a.k[j] : 0.f;
@@ -116,43 +114,36 @@ __global__ void __launch_bounds__(256) sepconv_col4_kernel(const ConvArgs a, int
   }
   __syncthreads();
 
-  float4 acc[RL];
+  float4 acc[kColRL];
 #pragma unroll
-  for (int r = 0; r < RL; ++r) acc[r] = zero4;
-  const float4* col = sm + (ty * RL) * 32 + tx;
-  float4 v[RL + 7];
+  for (int r = 0; r < kColRL; ++r) acc[r] = zero4;
+  const float4* col = sm + (ty * kColRL) * 32 + tx;
+  float4 v[kColRL + 7];
 #pragma unroll
-  for (int u = 0; u < 7; ++u) v[u] = u < RL + 7 ? col[u * 32] : zero4;
+  for (int u = 0; u < 7; ++u) v[u] = col[u * 32];
   for (int c = 0; c < Kp; c += 8) {
 #pragma unroll
-    for (int u = 7; u < RL + 7; ++u) v[u] = col[(c + u) * 32];
+    for (int u = 7; u < kColRL + 7; ++u) v[u] = col[(c + u) * 32];
     const float4 k0 = *reinterpret_cast<const float4*>(ks + c);
     const float4 k1 = *reinterpret_cast<const float4*>(ks + c + 4);
     const float kk[8] = {k0.x, k0.y, k0.z, k0.w, k1.x, k1.y, k1.z, k1.w};
 #pragma unroll
     for (int jj = 0; jj < 8; ++jj)
 #pragma unroll
-      for (int r = 0; r < RL; ++r) {
+      for (int r = 0; r < kColRL; ++r) {
         acc[r].x = fmaf(kk[jj], v[r + jj].x, acc[r].x);
         acc[r].y = fmaf(kk[jj], v[r + jj].y, acc[r].y);
         acc[r].z = fmaf(kk[jj], v[r + jj].z, acc[r].z);
         acc[r].w = fmaf(kk[jj], v[r + jj].w, acc[r].w);
       }
-    if (RL >= 8) {
 #pragma unroll
-      for (int u = 0; u < 7; ++u) v[u] = v[u + 8];
-    } else if (c + 8 < Kp) {
-      // RL < 8: the window is shorter than a chunk; the part of the next chunk's first 7 rows that is
-      // not in registers is loaded here (never past the last chunk: those rows are not staged)
-#pragma unroll
-      for (int u = 0; u < 7; ++u) v[u] = (u + 8 < RL + 7) ? v[u + 8] : col[(c + 8 + u) * 32];
-    }
+    for (int u = 0; u < 7; ++u) v[u] = v[u + 8];
   }
   if (!iok) return;
   float* oo = a.out + o * a.L_out * a.inner + i;
 #pragma unroll
-  for (int r = 0; r < RL; ++r) {
-    const int64_t l = l0 + ty * RL + r;
+  for (int r = 0; r < kColRL; ++r) {
+    const int64_t l = l0 + ty * kColRL + r;
     if (l < a.L_out) st_stream_f4(reinterpret_cast<float4*>(oo + l * a.inner), acc[r]);
   }
 }
@@ -265,24 +256,19 @@ int nrt_sepconv_axis_f32(const float* x, float* out, int64_t outer, int64_t L, i
   if (total == 0) return NRT_OK;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   ConvArgs a{x, out, kernel, outer, L, inner, L_out, K, stride, dilation, pad_before};
-  const char* env = getenv("NRT_CONV_GENERIC");
-  const bool force_generic = env && atoi(env) != 0;
+  const bool force_generic = env_int("NRT_CONV_GENERIC", 0) != 0;
   const int Kp = (K + 7) & ~7;
   const size_t col_smem = ((size_t)(kColTL + Kp - 1) * 32 + Kp) * sizeof(float);
   const int64_t halo = (int64_t)(K - 1) * dilation * inner;
   const size_t row_smem = (size_t)(kRowTP + halo + K) * sizeof(float);
-  const char* cenv = getenv("NRT_CONV_COL");           // 0: 32-wide tiles, 1: float4 x 32 outputs, 2: float4 x 64 outputs
-  const int col_mode = cenv ? atoi(cenv) : 2;
   if (!force_generic && stride == 1 && dilation == 1 && inner >= 32) {
-    const bool vec_ok = (inner % 4 == 0) && aligned16(x) && aligned16(out) && col_mode != 0;
-    const int TL4 = col_mode == 2 ? 64 : 32;
-    const size_t col4_smem = ((size_t)(TL4 + Kp - 1) * 128 + Kp) * sizeof(float);
+    const bool vec_ok = (inner % 4 == 0) && aligned16(x) && aligned16(out);
+    const size_t col4_smem = ((size_t)(kColTL + Kp - 1) * 128 + Kp) * sizeof(float);
     if (vec_ok && col4_smem <= 48 * 1024) {
-      const int64_t i_tiles = (inner + 127) / 128, l_tiles = (L_out + TL4 - 1) / TL4;
+      const int64_t i_tiles = (inner + 127) / 128, l_tiles = (L_out + kColTL - 1) / kColTL;
       const int64_t nblk = outer * i_tiles * l_tiles;
       NRT_REQUIRE(nblk <= 2147483647LL, NRT_E_SIZE, "tensor too large for one launch");
-      if (TL4 == 64) sepconv_col4_kernel<64><<<(unsigned)nblk, dim3(32, 8), col4_smem, st>>>(a, Kp, (int)i_tiles, (int)l_tiles);
-      else sepconv_col4_kernel<32><<<(unsigned)nblk, dim3(32, 8), col4_smem, st>>>(a, Kp, (int)i_tiles, (int)l_tiles);
+      sepconv_col4_kernel<<<(unsigned)nblk, dim3(32, 8), col4_smem, st>>>(a, Kp, (int)i_tiles, (int)l_tiles);
       return check_launch("sepconv_col4_kernel");
     }
     if (col_smem <= 48 * 1024) {

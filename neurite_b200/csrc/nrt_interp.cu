@@ -772,13 +772,13 @@ __device__ __forceinline__ void sample_global3(const float* __restrict__ volb, c
 // of the previous one.
 //   GENERAL = true : run-time `partial` (tile overhangs the output) and `has_fill` handling
 //   GENERAL = false: full tile, no fill value -- neither test exists in the loop
-template <int TZ, int TY, int HALO, int NW, int METHOD, int U, bool EZ, bool EY, bool EX, int CC, bool ABS, bool GENERAL>
+template <int TZ, int TY, int HALO, int METHOD, bool EZ, bool EY, bool EX, int CC, bool ABS, bool GENERAL>
 __device__ __forceinline__ void tile_rows(const float* __restrict__ s_flow, const float* __restrict__ s_box,
                                           const float* __restrict__ volb, float* __restrict__ outb,
                                           const TileGeo& w, int x0, int y0, int z0l, int ox, int oy, int oz,
                                           bool partial_rt) {
   using Cfg = TileCfg<TZ, TY, HALO, CC>;
-  constexpr int TX = Cfg::TX, BX = Cfg::BX, BY = Cfg::BY, BZ = Cfg::BZ;
+  constexpr int TX = Cfg::TX, BX = Cfg::BX, BY = Cfg::BY, BZ = Cfg::BZ, NW = Cfg::NW;
   constexpr int ZSTEP = NW >= TY ? NW / TY : 1;          // planes between a warp's rows
   constexpr int YROWS = NW >= TY ? 1 : TY / NW;          // rows per plane per warp
   const Geo& g = w.g;
@@ -809,7 +809,7 @@ __device__ __forceinline__ void tile_rows(const float* __restrict__ s_flow, cons
     bool all_ok = true;
     const float* fl0 = fl;
     float* op0 = op;
-#pragma unroll U
+#pragma unroll 2
     for (int z = zs; z < TZ; z += ZSTEP, fl += ZSTEP * TY * TX * 3, op += (size_t)ZSTEP * H * W * CC, zf += zstep) {
       if (partial && z >= nz_out) break;
       const float lz = __fadd_rn(zf, fl[0]);
@@ -895,18 +895,17 @@ __device__ __forceinline__ void tile_rows(const float* __restrict__ s_flow, cons
 // Process one staged tile.  Warp w owns row y = w % TY of planes z = w / TY, + NW/TY, ...
 // The per-axis EDGE flags are tile-uniform, so the dispatch below costs one uniform switch.  Tiles that overhang
 // the output and launches with a fill value take the one general variant (all edges, run-time checks).
-template <int TZ, int TY, int HALO, int NW, int METHOD, int U = 2, int CC = 1, bool ABS = false>
+template <int TZ, int TY, int HALO, int METHOD, int CC = 1, bool ABS = false>
 __device__ __forceinline__ void compute_tile(const float* __restrict__ s_flow, const float* __restrict__ s_box,
                                              const float* __restrict__ volb, float* __restrict__ outb,
                                              const TileGeo& w, int x0, int y0, int z0l, int ox, int oy, int oz) {
   using Cfg = TileCfg<TZ, TY, HALO, CC>;
-  static_assert(NW % TY == 0 || TY % NW == 0, "warps must tile the rows of a plane");
   const Geo& g = w.g;
   const bool ez = !((oz >= g.src_z0) && (oz + Cfg::BZ <= g.src_z0 + g.src_n0));
   const bool ey = !((oy >= 0) && (oy + Cfg::BY <= g.S[1]));
   const bool ex = !((ox >= 0) && (ox + Cfg::BX <= g.S[2]));
   const bool partial = (z0l + TZ > w.out_n0) || (y0 + TY > g.S[1]) || (x0 + Cfg::TX > g.S[2]);
-#define NRT_ROWS(a, b, c, gen) tile_rows<TZ, TY, HALO, NW, METHOD, U, a, b, c, CC, ABS, gen>(s_flow, s_box, volb, outb, w, x0, y0, z0l, ox, oy, oz, partial)
+#define NRT_ROWS(a, b, c, gen) tile_rows<TZ, TY, HALO, METHOD, a, b, c, CC, ABS, gen>(s_flow, s_box, volb, outb, w, x0, y0, z0l, ox, oy, oz, partial)
   if (partial || g.has_fill) { NRT_ROWS(true, true, true, true); return; }
   switch ((ez ? 4 : 0) | (ey ? 2 : 0) | (ex ? 1 : 0)) {
     case 0: NRT_ROWS(false, false, false, false); break;
@@ -926,8 +925,8 @@ __device__ __forceinline__ void compute_tile(const float* __restrict__ s_flow, c
 // with only 8-16 voxels per thread the prologue is a visible part of the instruction count.
 // ABS = the 'flow' tensor holds absolute sample locations (interpn on the volume's own grid): compile-time, so
 // that the displacement kernels carry no trace of it
-template <int TZ, int TY, int HALO, int METHOD, int U = 2, int NW = 8, int CC = 1, bool ABS = false>
-__global__ void __launch_bounds__(NW * 32)
+template <int TZ, int TY, int HALO, int METHOD, int CC = 1, bool ABS = false>
+__global__ void __launch_bounds__(TileCfg<TZ, TY, HALO, CC>::NW * 32)
 warp3d_tile_kernel(const __grid_constant__ CUtensorMap tm_vol,
                    const __grid_constant__ CUtensorMap tm_flow,
                    const float* __restrict__ vol, float* __restrict__ out, TileGeo w, int follow) {
@@ -1003,8 +1002,8 @@ warp3d_tile_kernel(const __grid_constant__ CUtensorMap tm_vol,
     }
     mbar_wait(bar, 1);
   }
-  compute_tile<TZ, TY, HALO, NW, METHOD, U, CC, ABS>(s_flow, s_box, vol + (size_t)b * w.src_batch_stride,
-                                                out + (size_t)b * w.out_bstride, w, x0, y0, z0l, ox, oy, oz);
+  compute_tile<TZ, TY, HALO, METHOD, CC, ABS>(s_flow, s_box, vol + (size_t)b * w.src_batch_stride,
+                                         out + (size_t)b * w.out_bstride, w, x0, y0, z0l, ox, oy, oz);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -1215,11 +1214,6 @@ static int encode_f32_4d(CUtensorMap* tm, const void* base, const uint64_t dims[
   return encode_f32_tiled(tm, base, 4, dims, box, batch_stride_elems);
 }
 
-int env_int(const char* name, int dflt) {
-  const char* s = getenv(name);
-  return (s && *s) ? atoi(s) : dflt;
-}
-
 int warp3d_bwd_tile(const float* vol, const float* flow, const float* gout, float* gvol, float* gflow, int B,
                     const int32_t* shape, int method, int has_fill, cudaStream_t st, bool* used) {
   *used = false;
@@ -1263,7 +1257,7 @@ int warp3d_bwd_tile(const float* vol, const float* flow, const float* gout, floa
   return check_launch("warp3d_bwd_tile_kernel");
 }
 
-template <int TZ, int TY, int HALO, int METHOD, int U = 2, int NW = 8, int CC = 1, bool ABS = false>
+template <int TZ, int TY, int HALO, int METHOD, int CC = 1, bool ABS = false>
 static int launch_tile(const float* vol, const float* flow, float* out, TileGeo tg, int H, int W, int src_n0,
                        int out_n0, cudaStream_t st) {
   using Cfg = TileCfg<TZ, TY, HALO, CC>;
@@ -1279,12 +1273,12 @@ static int launch_tile(const float* vol, const float* flow, float* out, TileGeo 
   if (rc != NRT_OK) return rc;
   rc = encode_f32_4d(&tmf, flow, fd, fb, (uint64_t)tg.flow_bstride);
   if (rc != NRT_OK) return rc;
-  auto kern = warp3d_tile_kernel<TZ, TY, HALO, METHOD, U, NW, CC, ABS>;
+  auto kern = warp3d_tile_kernel<TZ, TY, HALO, METHOD, CC, ABS>;
   // set on every launch: the attribute is per device and the call costs ~1 us of host time
   if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM) != cudaSuccess)
     return check_launch("cudaFuncSetAttribute(warp3d_tile)");
   const dim3 grid(tg.ntx, tg.nty, tg.ntz * tg.B);
-  kern<<<grid, NW * 32, Cfg::SMEM, st>>>(tmv, tmf, vol, out, tg, env_int("NRT_WARP_FOLLOW", 1));
+  kern<<<grid, Cfg::NW * 32, Cfg::SMEM, st>>>(tmv, tmf, vol, out, tg, env_int("NRT_WARP_FOLLOW", 1));
   return check_launch("warp3d_tile_kernel");
 }
 
@@ -1350,11 +1344,7 @@ static int try_tile_path(const float* vol, const float* flow, float* out, int B,
   const int H = shape[1], W = shape[2];
   if (env_int("NRT_WARP_TILE", 1) == 0) return NRT_OK;
   if (W % 4 != 0 || !aligned16(vol) || !aligned16(flow) || !aligned16(out) || W < 32) return NRT_OK;
-  // tile shapes (TZ x TY x 32) and halos built: the default 8x8x32 runs 4 CTAs per SM;
-  // `halo` picks the smallest built halo that covers it.
-  // 2: 8x8x32 (default), 3: 4x8x32
-  int cfg = env_int("NRT_WARP_TILE_CFG", 2);
-  if (cfg != 2 && cfg != 3) cfg = 2;
+  // C = 1 runs 8x8x32 tiles (4 CTAs per SM); `halo` picks the smallest built halo that covers it
   if (halo <= 0) halo = 3;
   const int hsel = halo <= 3 ? 3 : (halo <= 4 ? 4 : (halo <= 6 ? 6 : 8));
   TileGeo tg;
@@ -1375,8 +1365,8 @@ static int try_tile_path(const float* vol, const float* flow, float* out, int B,
 #define NRT_TILE_ABS(cc, tz)                                                                                 \
     if (C == (cc))                                                                                           \
       rc = method == NRT_LINEAR                                                                              \
-               ? launch_tile<tz, 8, 3, NRT_LINEAR, 2, 8, cc, true>(vol, flow, out, tg, H, W, src_n0, out_n0, st)   \
-               : launch_tile<tz, 8, 3, NRT_NEAREST, 2, 8, cc, true>(vol, flow, out, tg, H, W, src_n0, out_n0, st);
+               ? launch_tile<tz, 8, 3, NRT_LINEAR, cc, true>(vol, flow, out, tg, H, W, src_n0, out_n0, st)   \
+               : launch_tile<tz, 8, 3, NRT_NEAREST, cc, true>(vol, flow, out, tg, H, W, src_n0, out_n0, st);
     NRT_TILE_ABS(1, 8) NRT_TILE_ABS(2, 4) NRT_TILE_ABS(3, 4) NRT_TILE_ABS(4, 4)
 #undef NRT_TILE_ABS
     if (rc == 1) return NRT_OK;
@@ -1389,21 +1379,20 @@ static int try_tile_path(const float* vol, const float* flow, float* out, int B,
 #define NRT_TILE_C(cc)                                                                                   \
     if (C == (cc))                                                                                       \
       rc = method == NRT_LINEAR                                                                          \
-               ? launch_tile<4, 8, 3, NRT_LINEAR, 2, 8, cc>(vol, flow, out, tg, H, W, src_n0, out_n0, st)  \
-               : launch_tile<4, 8, 3, NRT_NEAREST, 2, 8, cc>(vol, flow, out, tg, H, W, src_n0, out_n0, st);
+               ? launch_tile<4, 8, 3, NRT_LINEAR, cc>(vol, flow, out, tg, H, W, src_n0, out_n0, st)  \
+               : launch_tile<4, 8, 3, NRT_NEAREST, cc>(vol, flow, out, tg, H, W, src_n0, out_n0, st);
     NRT_TILE_C(2) NRT_TILE_C(3) NRT_TILE_C(4)
 #undef NRT_TILE_C
     if (rc == 1) return NRT_OK;
     *used = true;
     return rc;
   }
-#define NRT_TILE_CASE(i, tz, ty, hh)                                                                     \
-  if (cfg == (i) && hsel == (hh))                                                                        \
+#define NRT_TILE_CASE(hh)                                                                                \
+  if (hsel == (hh))                                                                                      \
     rc = method == NRT_LINEAR                                                                            \
-             ? launch_tile<tz, ty, hh, NRT_LINEAR>(vol, flow, out, tg, H, W, src_n0, out_n0, st)         \
-             : launch_tile<tz, ty, hh, NRT_NEAREST>(vol, flow, out, tg, H, W, src_n0, out_n0, st);
-  NRT_TILE_CASE(2, 8, 8, 3) NRT_TILE_CASE(2, 8, 8, 4) NRT_TILE_CASE(2, 8, 8, 6) NRT_TILE_CASE(2, 8, 8, 8)
-  NRT_TILE_CASE(3, 4, 8, 3) NRT_TILE_CASE(3, 4, 8, 4) NRT_TILE_CASE(3, 4, 8, 6) NRT_TILE_CASE(3, 4, 8, 8)
+             ? launch_tile<8, 8, hh, NRT_LINEAR>(vol, flow, out, tg, H, W, src_n0, out_n0, st)           \
+             : launch_tile<8, 8, hh, NRT_NEAREST>(vol, flow, out, tg, H, W, src_n0, out_n0, st);
+  NRT_TILE_CASE(3) NRT_TILE_CASE(4) NRT_TILE_CASE(6) NRT_TILE_CASE(8)
 #undef NRT_TILE_CASE
   if (rc == 1) return NRT_OK;                              // not launched: fall back
   *used = true;
@@ -1492,8 +1481,7 @@ static int warp_impl(const float* vol, const float* flow, float* out, int B, con
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   // 3 or more channels: z-marching ring kernel (all channels of a voxel side by side in shared memory); C = 2 stays
   // on the box tiles, whose halo is still small at two channels.
-  const int march_min_c = env_int("NRT_MARCH_SMALLC", 0) ? 2 : env_int("NRT_MARCH_MINC", 3);
-  if (D == 3 && C >= 2 && C >= march_min_c) {
+  if (D == 3 && C >= 3) {
     bool used = false;
     rc = warp3d_march(vol, flow, out, B, shape, C, method, has_fill, fill, src_z0, src_n0, out_z0, out_n0,
                       halo, err_flag, vbs, fbs, obs, st, &used);
@@ -1557,12 +1545,10 @@ int nrt_resize_f32(const float* vol, float* out, int B, const int32_t* in_shape,
   rg.out_vox = out_plane * out_n0;
   if (B == 0 || rg.out_vox == 0) return NRT_OK;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (D == 3 && in_vox * C <= 0x7fffffffLL && getenv("NRT_RESIZE_GENERIC") == nullptr) {
-    const char* tze = getenv("NRT_RESIZE_TZ");
+  if (D == 3 && in_vox * C <= 0x7fffffffLL && env_int("NRT_RESIZE_GENERIC", 0) == 0) {
     // planes per CTA: 32 (fewer prologues and box waits per output plane); short slabs take fewer so that the grid
     // keeps a few waves
-    int TZ = tze ? atoi(tze) : (out_n0 >= 64 ? 32 : (out_n0 >= 24 ? 16 : 8));
-    if (TZ != 16 && TZ != 32 && TZ != 64) TZ = 8;
+    int TZ = out_n0 >= 64 ? 32 : (out_n0 >= 24 ? 16 : 8);
     if (method != NRT_LINEAR || C < 1 || C > 4) TZ = 8;          // the marching path is linear, C = 1..4
     // up-sampling: source box of every output tile staged by TMA (resize3d_tile_kernel)
     if (method == NRT_LINEAR && C >= 1 && C <= 4 && env_int("NRT_RESIZE_TILE", 1) && aligned16(vol) &&
@@ -1579,10 +1565,9 @@ int nrt_resize_f32(const float* vol, float* out, int B, const int32_t* in_shape,
       bxs.by = resize_axis_extent(rg.g.S[1], rg.M[1], rg.delta[1], 0, rg.M[1], tyt, 1);
       bxs.bx = resize_axis_extent(rg.g.S[2], rg.M[2], rg.delta[2], 0, rg.M[2], 32, xalign);
       bxs.bx = (bxs.bx + xalign - 1) / xalign * xalign;
-      const int tzt = (TZ == 64) ? 32 : TZ;
-      bxs.bz = resize_axis_extent(rg.g.S[0], rg.M[0], rg.delta[0], out_z0, out_n0, tzt, 1);
+      bxs.bz = resize_axis_extent(rg.g.S[0], rg.M[0], rg.delta[0], out_z0, out_n0, TZ, 1);
       const size_t box_bytes = (size_t)bxs.bz * bxs.by * bxs.bx * C * 4;
-      const int ntz3 = (out_n0 + tzt - 1) / tzt, nty3 = (rg.M[1] + tyt - 1) / tyt, ntx3 = (rg.M[2] + 31) / 32;
+      const int ntz3 = (out_n0 + TZ - 1) / TZ, nty3 = (rg.M[1] + tyt - 1) / tyt, ntx3 = (rg.M[2] + 31) / 32;
       const int64_t grid3 = (int64_t)B * ntz3 * nty3 * ntx3;
       if (box_bytes <= box_budget && bxs.bx * C <= 256 && bxs.by <= 256 && bxs.bz <= 256 && grid3 <= 0x7fffffffLL) {
         CUtensorMap tmv;
@@ -1611,7 +1596,7 @@ int nrt_resize_f32(const float* vol, float* out, int B, const int32_t* in_shape,
           }                                                                                                               \
         } while (0)
 #define NRT_RESIZE_TILE_C(CT)                                                                                             \
-        do { if (tzt == 8) NRT_RESIZE_TILE(CT, 8); else if (tzt == 16) NRT_RESIZE_TILE(CT, 16); else NRT_RESIZE_TILE(CT, 32); } while (0)
+        do { if (TZ == 8) NRT_RESIZE_TILE(CT, 8); else if (TZ == 16) NRT_RESIZE_TILE(CT, 16); else NRT_RESIZE_TILE(CT, 32); } while (0)
         switch (C) {
           case 1: NRT_RESIZE_TILE_C(1); break;
           case 2: NRT_RESIZE_TILE_C(2); break;
@@ -1631,7 +1616,6 @@ int nrt_resize_f32(const float* vol, float* out, int B, const int32_t* in_shape,
         if (method != NRT_LINEAR) resize3d_kernel<NRT_NEAREST, CT><<<(int)grid, 256, 0, st>>>(vol, out, rg, ntz, nty, ntx);  \
         else if (TZ == 16) resize3d_kernel<NRT_LINEAR, CT, 16><<<(int)grid, 256, 0, st>>>(vol, out, rg, ntz, nty, ntx);     \
         else if (TZ == 32) resize3d_kernel<NRT_LINEAR, CT, 32><<<(int)grid, 256, 0, st>>>(vol, out, rg, ntz, nty, ntx);     \
-        else if (TZ == 64) resize3d_kernel<NRT_LINEAR, CT, 64><<<(int)grid, 256, 0, st>>>(vol, out, rg, ntz, nty, ntx);     \
         else resize3d_kernel<NRT_LINEAR, CT><<<(int)grid, 256, 0, st>>>(vol, out, rg, ntz, nty, ntx); \
       } while (0)
       // the C = 2 / 4 kernels store float2 / float4 per voxel: fall back to the run-time-C kernel for an unaligned output

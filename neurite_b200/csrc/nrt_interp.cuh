@@ -236,8 +236,6 @@ __device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) {
 }
 
 
-int env_int(const char* name, int dflt);
-
 // multi-channel D = 3 warp through the z-marching ring kernel (nrt_warp_march.cu); *used = false when not covered
 int warp3d_march(const float* vol, const float* flow, float* out, int B, const int32_t* shape, int C, int method,
                  int has_fill, float fill, int src_z0, int src_n0, int out_z0, int out_n0, int halo,

@@ -539,8 +539,7 @@ static int launch_stream(const float* x, const float* kernel, const float* bias,
     return check_launch("cudaFuncSetAttribute(lc3d_stream)");
   int grid = sm_count();
   if (g.pn < grid) grid = (int)g.pn;
-  int nw = kLcMaxWarps;                          // as many consumer groups as the ring allows (measured best)
-  if (const char* e = getenv("NRT_LC3D_WARPS")) nw = atoi(e);
+  int nw = env_int("NRT_LC3D_WARPS", kLcMaxWarps);   // as many consumer groups as the ring allows (measured best)
   if (nw < 1) nw = 1;
   if (nw > kLcMaxWarps) nw = kLcMaxWarps;
   if (nw > stages - 1) nw = stages - 1;
@@ -563,7 +562,8 @@ static int launch_patch(const float* x, const float* kernel, const float* bias, 
   int stages = (int)((220 * 1024 - 2 * kLcMaxStages * sizeof(uint64_t) - 128) / (size_t)slot_stride);
   if (stages < 3) return 1;
   if (stages > kLcMaxStages) stages = kLcMaxStages;
-  if (const char* e = getenv("NRT_LC3D_STAGES")) { const int s = atoi(e); if (s >= 3 && s < stages) stages = s; }
+  const int forced_stages = env_int("NRT_LC3D_STAGES", 0);
+  if (forced_stages >= 3 && forced_stages < stages) stages = forced_stages;
   const size_t smem = (size_t)stages * slot_stride + (size_t)stages * 16 + 16;
   CUtensorMap tmx;
   const uint64_t xd[5] = {(uint64_t)g.Cin, (uint64_t)g.I[2], (uint64_t)g.I[1], (uint64_t)g.I[0], (uint64_t)g.B};
@@ -575,8 +575,7 @@ static int launch_patch(const float* x, const float* kernel, const float* bias, 
     return check_launch("cudaFuncSetAttribute(lc3d_patch)");
   int grid = sm_count();
   if (g.pn < grid) grid = (int)g.pn;
-  int nw = kLcMaxWarps;
-  if (const char* e = getenv("NRT_LC3D_WARPS")) nw = atoi(e);
+  int nw = env_int("NRT_LC3D_WARPS", kLcMaxWarps);
   if (nw < 1) nw = 1;
   if (nw > kLcMaxWarps) nw = kLcMaxWarps;
   if (nw > stages - 1) nw = stages - 1;
@@ -600,7 +599,8 @@ static int launch_rows(const float* x, const float* kernel, const float* bias, f
   int stages = (int)((220 * 1024 - 2 * kLcMaxStages * sizeof(uint64_t) - 128) / (size_t)slot_stride);
   if (stages < 3) return 1;
   if (stages > kLcMaxStages) stages = kLcMaxStages;
-  if (const char* e = getenv("NRT_LC3D_STAGES")) { const int s = atoi(e); if (s >= 3 && s < stages) stages = s; }
+  const int forced_stages = env_int("NRT_LC3D_STAGES", 0);
+  if (forced_stages >= 3 && forced_stages < stages) stages = forced_stages;
   const size_t smem = (size_t)stages * slot_stride + (size_t)stages * 16 + 16;
   CUtensorMap tmx;
   const uint64_t xd[5] = {(uint64_t)g.Cin, (uint64_t)g.I[2], (uint64_t)g.I[1], (uint64_t)g.I[0], (uint64_t)g.B};
@@ -612,8 +612,7 @@ static int launch_rows(const float* x, const float* kernel, const float* bias, f
     return check_launch("cudaFuncSetAttribute(lc3d_rows)");
   int grid = sm_count();
   if (g.pn < grid) grid = (int)g.pn;
-  int nw = kLcMaxWarps;                          // consumer groups: as many as the ring allows, one slot left in flight
-  if (const char* e = getenv("NRT_LC3D_WARPS")) nw = atoi(e);
+  int nw = env_int("NRT_LC3D_WARPS", kLcMaxWarps);   // consumer groups: as many as the ring allows, one slot left in flight
   if (nw < 1) nw = 1;
   if (nw > kLcMaxWarps) nw = kLcMaxWarps;
   if (nw > stages - 1) nw = stages - 1;
@@ -655,7 +654,7 @@ extern "C" int nrt_lc3d_fwd_f32(const float* x, const float* kernel, const float
   const int cq = Cout / 4;
   const bool fast = (Cout % 4 == 0) && cq <= 32 && (cq & (cq - 1)) == 0 && aligned16(kernel) && aligned16(out) &&
                     (!bias || aligned16(bias)) && ((int64_t)g.F * Cout * 4) % 16 == 0 && g.F <= 8192 &&
-                    getenv("NRT_LC3D_GENERIC") == nullptr;
+                    env_int("NRT_LC3D_GENERIC", 0) == 0;
   if (fast) {
     int cq_log2 = 0;
     while ((1 << cq_log2) < cq) ++cq_log2;

@@ -18,7 +18,6 @@
 // probability maps (segs) it streams 8*nb bytes per voxel and is HBM-bound.
 #include "nrt_common.cuh"
 
-#include <cstdlib>
 #include <math.h>
 
 namespace nrt {
@@ -556,23 +555,18 @@ __global__ void soft_quantize_kernel(const float* x, int64_t n, const float* cen
   }
 }
 
-template <int MT, int NT, int SPCQ, int SPCM>
-void launch_mma(const MiArgs& a, dim3 grid, cudaStream_t st, int variant) {
-  if (a.x.quant && a.y.quant) {
-    // 2 CTAs per SM: the MUFU and tensor pipes are the limit, more resident warps only add contention.
-    // NRT_MI_VARIANT (dev switch):
-    // 1 = 2 steps per chunk at 3 CTAs per SM, 2 = 4 steps at 3 CTAs per SM
-    if (variant == 1) mi_hist_mma_kernel<MT, NT, true, true, 2, 3><<<grid, kMiThreads, 0, st>>>(a);
-    else if (variant == 2) mi_hist_mma_kernel<MT, NT, true, true, SPCQ, 3><<<grid, kMiThreads, 0, st>>>(a);
-    else mi_hist_mma_kernel<MT, NT, true, true, SPCQ, 2><<<grid, kMiThreads, 0, st>>>(a);
-  } else if (a.x.quant) mi_hist_mma_kernel<MT, NT, true, false, SPCM><<<grid, kMiThreads, 0, st>>>(a);
-  else if (a.y.quant) mi_hist_mma_kernel<MT, NT, false, true, SPCM><<<grid, kMiThreads, 0, st>>>(a);
-  else mi_hist_mma_kernel<MT, NT, false, false, SPCM><<<grid, kMiThreads, 0, st>>>(a);
+template <int MT, int NT, int SPC>
+void launch_mma(const MiArgs& a, dim3 grid, cudaStream_t st) {
+  // two quantised operands: 2 CTAs per SM -- the MUFU and tensor pipes are the limit, more resident warps only add
+  // contention
+  if (a.x.quant && a.y.quant) mi_hist_mma_kernel<MT, NT, true, true, SPC, 2><<<grid, kMiThreads, 0, st>>>(a);
+  else if (a.x.quant) mi_hist_mma_kernel<MT, NT, true, false, SPC><<<grid, kMiThreads, 0, st>>>(a);
+  else if (a.y.quant) mi_hist_mma_kernel<MT, NT, false, true, SPC><<<grid, kMiThreads, 0, st>>>(a);
+  else mi_hist_mma_kernel<MT, NT, false, false, SPC><<<grid, kMiThreads, 0, st>>>(a);
 }
 
 int mi_blocks(int64_t nv, int items) {
-  const char* be = getenv("NRT_MI_CTAS_PER_SM");
-  const int per_sm = be ? atoi(be) : 4;
+  const int per_sm = env_int("NRT_MI_CTAS_PER_SM", 4);
   int64_t want = ((int64_t)sm_count() * (per_sm > 0 ? per_sm : 4) + items - 1) / items;          // ~4 CTAs per SM in total
   int64_t cap = (nv + 1023) / 1024;                                      // >= 1024 voxels per CTA
   int64_t n = want < cap ? want : cap;
@@ -624,17 +618,14 @@ int nrt_mi_hist_f32(const float* x, int64_t x_batch_stride, int64_t x_vox_stride
   const int nblk = mi_blocks(nv, items);
   a.nblk = nblk;
   dim3 grid(nblk, C, B);
-  const char* venv = getenv("NRT_MI_VARIANT");
-  const int variant = venv ? atoi(venv) : 0;
-  const char* env = getenv("NRT_MI_GENERIC");
   // alpha <= 0 would turn the padded bins' exp(-alpha * inf) into NaN: no padding in the generic kernel
-  const bool generic = (env && atoi(env) != 0) || nbx > 32 || nby > 32 || !(alpha > 0.f);
+  const bool generic = env_int("NRT_MI_GENERIC", 0) != 0 || nbx > 32 || nby > 32 || !(alpha > 0.f);
   if (generic) {
     mi_hist_generic_kernel<<<grid, kMiThreads, 0, st>>>(a);
   } else if (nbx <= 16 && nby <= 16) {
-    launch_mma<1, 2, 4, 4>(a, grid, st, variant);
+    launch_mma<1, 2, 4>(a, grid, st);
   } else {
-    launch_mma<2, 4, 2, 2>(a, grid, st, 0);          // 32 x 32 bins: 64 accumulators, 2 CTAs per SM
+    launch_mma<2, 4, 2>(a, grid, st);                // 32 x 32 bins: 64 accumulators, 2 CTAs per SM
   }
   int rc = check_launch("mi_hist kernel");
   if (rc != NRT_OK) return rc;

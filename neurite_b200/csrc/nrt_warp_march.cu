@@ -34,9 +34,8 @@ struct MarchGeo {
 // CCH = channels staged per voxel (a chunk of the volume's C); VEC: lanes own 4-channel quads, else all CCH channels.
 // QPT = quads per thread (VEC only): the per-voxel corner setup (~60 instructions) and the 8 corner weights are
 // shared by the QPT quads a thread owns -- with one quad per thread they are 2/3 of all instructions.
-// G = output planes in flight per CTA (plane groups of NW / G warps each, see the kernel): the ring then holds the
-// windows of G consecutive output planes plus AHEAD planes of prefetch.
-template <int CCH, int TY_, int TX_, int HALO_, int AHEAD_, int QPT_ = 1, int G_ = 1>
+// The ring holds the window of one output plane plus AHEAD planes of prefetch.
+template <int CCH, int TY_, int TX_, int HALO_, int AHEAD_, int QPT_ = 1>
 struct MarchCfg {
   static constexpr int TY = TY_, TX = TX_, HALO = HALO_, AHEAD = AHEAD_;
   static constexpr bool VEC = (CCH % 4 == 0);
@@ -46,10 +45,10 @@ struct MarchCfg {
   static constexpr int CPL = VEC ? 4 : CCH;                     // channels per lane and pass
   static_assert(!VEC || Q % QPT == 0, "quads per thread must divide the quads per voxel");
   // the TMA needs a 16-byte aligned start address: (x0 - HX) * C * 4 bytes
-  static constexpr int HX = VEC ? HALO : ((CCH % 2 == 0) ? ((HALO + 1) & ~1) : ((HALO + 3) & ~3));
+  static constexpr int HX = VEC ? HALO : ((HALO + 3) & ~3);
   static constexpr int BY = TY + 2 * HALO, BX = TX + 2 * HX;
   static constexpr int WIN = 2 * HALO + 1;                      // source planes one output plane can touch
-  static constexpr int R = WIN + (G_ - 1) + AHEAD;              // ring slots
+  static constexpr int R = WIN + AHEAD;                         // ring slots
   static constexpr int BOX_ELEMS = BY * BX * CCH, FLOW_ELEMS = TY * TX * 3;
   static constexpr int BOX_BYTES = BOX_ELEMS * 4, FLOW_BYTES = FLOW_ELEMS * 4;
   static constexpr int FLOW_OFF = (BOX_BYTES + 127) & ~127;     // byte offset of the flow tile inside a slot
@@ -71,18 +70,13 @@ __device__ __forceinline__ void lds_channels(const float* p, float (&v)[CPL]) {
   }
 }
 
-template <int CCH, int TY, int TX, int HALO, int AHEAD, int NW, int METHOD, int QPT = 1, int G = 1>
+template <int CCH, int TY, int TX, int HALO, int AHEAD, int NW, int METHOD, int QPT = 1>
 __global__ void __launch_bounds__((NW + 1) * 32, 1)
 warp3d_march_kernel(const __grid_constant__ CUtensorMap tm_vol, const __grid_constant__ CUtensorMap tm_flow,
                     const float* __restrict__ vol, float* __restrict__ out, MarchGeo w) {
-  using Cfg = MarchCfg<CCH, TY, TX, HALO, AHEAD, QPT, G>;
+  using Cfg = MarchCfg<CCH, TY, TX, HALO, AHEAD, QPT>;
   constexpr int R = Cfg::R, WIN = Cfg::WIN, BX = Cfg::BX, BY = Cfg::BY, LPV = Cfg::LPV, CPL = Cfg::CPL, Q = Cfg::Q;
-  // Plane groups: the NW consumer warps form G groups of NW / G warps; group p produces the output planes j = p, p + G,
-  // ... of the column, so G consecutive output planes are in flight (twice the warps per SM for the same plane tile:
-  // with two quads per thread one plane occupies only 8 warps).  Every warp releases ring index i exactly once: after
-  // its output j it is done with the indices j .. j + G - 1 (its next output starts at j + G).
-  static_assert(NW % G == 0 && G >= 1 && G <= WIN, "plane groups");
-  constexpr int NTC = (NW / G) * 32;
+  constexpr int NTC = NW * 32;
   static_assert(Cfg::ITEMS % NTC == 0, "the plane tile must be a whole number of passes of the consumer threads");
   constexpr int ITER = Cfg::ITEMS / NTC;
   extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -141,16 +135,12 @@ warp3d_march_kernel(const __grid_constant__ CUtensorMap tm_vol, const __grid_con
     const int v = item / LPV;
     vxs[it] = v % TX; vys[it] = v / TX;
   }
-  const int grp = wid / (NW / G);
-  if (G > 1 && lane == 0) {
-    // ring indices below the group's first output have no output of this group behind them: release them up front
-    for (int i = 0; i < grp; ++i) mbar_arrive(empty + (i % R));
-  }
-  for (int j = grp; j < nz; j += G) {
+  // every warp waits for every ring index in increasing order, so a barrier is never more than one phase ahead:
+  // the first 2 HALO planes once, then the newest plane of each output plane's window
+  for (int i = 0; i < 2 * HALO; ++i) mbar_wait(full + i, 0);
+  for (int j = 0; j < nz; ++j) {
     const int inew = j + 2 * HALO;
-    // wait for the planes of this window the warp has not seen yet (all of them at its first output, G afterwards);
-    // every warp waits for every ring index in increasing order, so a barrier is never more than one phase ahead
-    for (int i = (j == grp ? j : inew - G + 1); i <= inew; ++i) mbar_wait(full + (i % R), (uint32_t)((i / R) & 1));
+    mbar_wait(full + (inew % R), (uint32_t)((inew / R) & 1));
     const int wbase = j % R;                                    // ring slot of the window's first plane
     const float* s_flow = reinterpret_cast<const float*>(smem_raw + (size_t)(inew % R) * Cfg::SLOT_BYTES + Cfg::FLOW_OFF);
     const int zl = zs + j, gz = w.out_z0 + zl;
@@ -258,18 +248,15 @@ warp3d_march_kernel(const __grid_constant__ CUtensorMap tm_vol, const __grid_con
         for (int c = 0; c < CPL; ++c) op[c] = res[0][c];
       }
     }
-    // this warp is done with the oldest G planes of the window (its next output plane is j + G)
+    // this warp is done with the oldest plane of the window (its next output plane is j + 1)
     __syncwarp();
-    if (lane == 0) {
-#pragma unroll
-      for (int i = 0; i < G; ++i) mbar_arrive(empty + ((j + i) % R));
-    }
+    if (lane == 0) mbar_arrive(empty + (j % R));
   }
 }
 
-template <int CCH, int TY, int TX, int HALO, int AHEAD, int NW, int METHOD, int QPT = 1, int G = 1>
+template <int CCH, int TY, int TX, int HALO, int AHEAD, int NW, int METHOD, int QPT = 1>
 static int launch_march(const float* vol, const float* flow, float* out, MarchGeo mg, cudaStream_t st) {
-  using Cfg = MarchCfg<CCH, TY, TX, HALO, AHEAD, QPT, G>;
+  using Cfg = MarchCfg<CCH, TY, TX, HALO, AHEAD, QPT>;
   static_assert(Cfg::SMEM <= 227 * 1024, "ring does not fit shared memory");
   const int H = mg.g.S[1], W = mg.g.S[2], C = mg.g.C;
   const int ntx = (W + TX - 1) / TX, nty = (H + TY - 1) / TY;
@@ -300,7 +287,7 @@ static int launch_march(const float* vol, const float* flow, float* out, MarchGe
   const uint32_t fb[4] = {(uint32_t)TX * 3, (uint32_t)TY, 1, 1};
   rc = encode_f32_tiled(&tmf, flow, 4, fd, fb, (uint64_t)mg.flow_bstride);
   if (rc != NRT_OK) return rc;
-  auto kern = warp3d_march_kernel<CCH, TY, TX, HALO, AHEAD, NW, METHOD, QPT, G>;
+  auto kern = warp3d_march_kernel<CCH, TY, TX, HALO, AHEAD, NW, METHOD, QPT>;
   if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM) != cudaSuccess)
     return check_launch("cudaFuncSetAttribute(warp3d_march)");
   const dim3 grid(ntx, nty, (unsigned)gz);
@@ -329,36 +316,21 @@ int warp3d_march(const float* vol, const float* flow, float* out, int B, const i
   mg.flow_bstride = fbs ? fbs : mg.out_vox * 3;
   mg.out_bstride = obs ? obs : mg.out_vox * C;
   if ((mg.src_batch_stride | mg.flow_bstride | mg.out_bstride) & 3) return NRT_OK;   // TMA strides: multiples of 16 bytes
+  const bool lin = method == NRT_LINEAR;
   int rc = 1;
-  const int nw16 = env_int("NRT_MARCH_NW", 16);
-  // quads per thread: 2 by default for 8 / 16-channel chunks (the corner setup is shared by two quads; i.i.d. flows
-  // are bank-conflict bound either way)
-  const int qpt = env_int("NRT_MARCH_QPT", 2);
-#define NRT_MARCH(cch, ty, tx, ahead, nw)                                                                      \
-  rc = method == NRT_LINEAR ? launch_march<cch, ty, tx, 3, ahead, nw, NRT_LINEAR>(vol, flow, out, mg, st)      \
-                            : launch_march<cch, ty, tx, 3, ahead, nw, NRT_NEAREST>(vol, flow, out, mg, st)
-#define NRT_MARCH_Q(cch, ty, tx, ahead, nw, qq)                                                                \
-  rc = method == NRT_LINEAR ? launch_march<cch, ty, tx, 3, ahead, nw, NRT_LINEAR, qq>(vol, flow, out, mg, st)  \
-                            : launch_march<cch, ty, tx, 3, ahead, nw, NRT_NEAREST, qq>(vol, flow, out, mg, st)
-  // (two output planes in flight per CTA -- template parameter G = 2 -- is not instantiated: the kernel is not short
-  // of warps.)
-  if (C % 16 == 0) {
-    // QPT 2 / 4: a thread owns 8 / 16 channels of its voxel and shares the corner setup between them
-    if (qpt == 4) NRT_MARCH_Q(16, 8, 16, 3, 4, 4);
-    else if (qpt == 2) NRT_MARCH_Q(16, 8, 16, 3, 8, 2);
-    else if (nw16 == 8) NRT_MARCH(16, 8, 16, 3, 8); else NRT_MARCH(16, 8, 16, 3, 16);
-  } else if (C % 8 == 0) {
-    if (qpt >= 2) NRT_MARCH_Q(8, 8, 32, 3, 8, 2);
-    else if (nw16 == 8) NRT_MARCH(8, 8, 32, 3, 8); else NRT_MARCH(8, 8, 32, 3, 16);
-  } else if (C % 4 == 0) {
-    if (nw16 == 8) NRT_MARCH(4, 16, 32, 3, 8); else NRT_MARCH(4, 16, 32, 3, 16);
-  } else if (C == 3 && env_int("NRT_MARCH_C3", 1)) {
-    NRT_MARCH(3, 8, 32, 3, 8);
-  } else if (C == 2 && env_int("NRT_MARCH_C2", 1)) {
-    NRT_MARCH(2, 16, 32, 3, 16);
-  }
-#undef NRT_MARCH_Q
-#undef NRT_MARCH
+  // 8 / 16-channel chunks: two quads per thread share the corner setup (i.i.d. flows are bank-conflict bound either way)
+  if (C % 16 == 0)
+    rc = lin ? launch_march<16, 8, 16, 3, 3, 8, NRT_LINEAR, 2>(vol, flow, out, mg, st)
+             : launch_march<16, 8, 16, 3, 3, 8, NRT_NEAREST, 2>(vol, flow, out, mg, st);
+  else if (C % 8 == 0)
+    rc = lin ? launch_march<8, 8, 32, 3, 3, 8, NRT_LINEAR, 2>(vol, flow, out, mg, st)
+             : launch_march<8, 8, 32, 3, 3, 8, NRT_NEAREST, 2>(vol, flow, out, mg, st);
+  else if (C % 4 == 0)
+    rc = lin ? launch_march<4, 16, 32, 3, 3, 16, NRT_LINEAR>(vol, flow, out, mg, st)
+             : launch_march<4, 16, 32, 3, 3, 16, NRT_NEAREST>(vol, flow, out, mg, st);
+  else if (C == 3)
+    rc = lin ? launch_march<3, 8, 32, 3, 3, 8, NRT_LINEAR>(vol, flow, out, mg, st)
+             : launch_march<3, 8, 32, 3, 3, 8, NRT_NEAREST>(vol, flow, out, mg, st);
   if (rc == 1) return NRT_OK;
   *used = true;
   return rc;

@@ -6,7 +6,7 @@ with the fp64 graphs of oracle/grad.py, oracle/mi.py and oracle/forward.py withi
 oracle.forward.value_close:  |got - ref| <= 4 k 2^-24 scale + approx.  scale is the sum of the absolute terms of
 the element, k the fp32 rounding depth the kernel's launch geometry gives it, approx the documented error of an
 approximate function (named in oracle/forward.py).  Each case names the kernel it is meant to reach;
-test_forward_dispatch_reaches_each_kernel checks that it does.
+test_forward_dispatch_launches_each_kernel checks that it does.
 """
 import ctypes
 import re
@@ -390,15 +390,13 @@ def _mi_operand(g, kind, B, nv, C, nb, base=None):
     return torch.softmax(z, -1)
 
 
-def _mi_spc(nbx, nby, qq, env):
-    """8-voxel MMA steps per chunk of the instantiation launch_mma picks (NRT_MI_VARIANT=1: 2)."""
-    if max(nbx, nby) > 16:
-        return 2
-    return 2 if qq and env.get('NRT_MI_VARIANT') == '1' else 4
+def _mi_spc(nbx, nby):
+    """8-voxel MMA steps per chunk of the instantiation launch_mma picks."""
+    return 2 if max(nbx, nby) > 16 else 4
 
 
 def _mi_case(ne, x, xq, nbx, y, yq, nby, B, C, nv, alpha=None, lo=-np.inf, hi=np.inf, centers=None, generic=False,
-             per_sm=None, env=None, tag=''):
+             per_sm=None, tag=''):
     """Run the ABI on x, y; check every stats element and the MI against the fp64 reference."""
     if alpha is None:
         alpha = float(ne.metrics.MutualInformation(nb_bins=max(nbx if xq else nby, 2)).soft_bin_alpha)
@@ -422,7 +420,7 @@ def _mi_case(ne, x, xq, nbx, y, yq, nby, B, C, nv, alpha=None, lo=-np.inf, hi=np
     wy, ey = w(y, yq, cyh, nby)
     tc = not generic and nbx <= 32 and nby <= 32
     ref, approx = of.mi_hist_reference(wx, ex, wy, ey, tc)
-    kh, km = of.mi_hist_depth(nv, B * C, nbx, nby, not tc, _mi_spc(nbx, nby, xq and yq, env or {}), per_sm=per_sm)
+    kh, km = of.mi_hist_depth(nv, B * C, nbx, nby, not tc, _mi_spc(nbx, nby), per_sm=per_sm)
     npair = nbx * nby
     k = torch.full((stats.shape[1],), float(km), device='cuda')
     k[:npair] = kh
@@ -436,8 +434,7 @@ def _mi_case(ne, x, xq, nbx, y, yq, nby, B, C, nv, alpha=None, lo=-np.inf, hi=np
 # (name, x kind, nbx, y kind, nby, channels, env)
 MI_CASES = [
     ('mma12-qq-v0', 'q', 16, 'q', 16, 1, {}),
-    ('mma12-qq-v1', 'q', 16, 'q', 16, 1, {'NRT_MI_VARIANT': '1'}),
-    ('mma12-qq-v2', 'q', 11, 'q', 11, 1, {'NRT_MI_VARIANT': '2'}),
+    ('mma12-qq-v2', 'q', 11, 'q', 11, 1, {}),
     ('mma12-qq-c3', 'q', 16, 'q', 16, 3, {}),
     ('mma24-qq', 'q', 32, 'q', 32, 1, {}),
     ('mma12-qm', 'q', 16, 'm', 16, 1, {}),
@@ -457,7 +454,7 @@ MI_CASES = [
 @pytest.mark.parametrize('nv', [1, 127, 128, 129, 2 ** 17 + 13])
 @pytest.mark.parametrize('name,xk,nbx,yk,nby,C,env', MI_CASES, ids=[c[0] for c in MI_CASES])
 def test_mi_hist_vs_fp64_reference(ne, monkeypatch, name, xk, nbx, yk, nby, C, env, nv):
-    """mi_hist_mma_kernel <1,2> (NRT_MI_VARIANT 0, 1, 2) and <2,4> for every quantisation combination, including
+    """mi_hist_mma_kernel <1,2> and <2,4> for every quantisation combination, including
     the y-only one and nbx != nby (16x5, 32x12) that only the C ABI reaches; mi_hist_generic_kernel (> 32 bins,
     NRT_MI_GENERIC=1); NRT_MI_CTAS_PER_SM 1, 2, 8; voxel counts around the 128-voxel flush and many CTAs."""
     for kv in env.items():
@@ -468,7 +465,7 @@ def test_mi_hist_vs_fp64_reference(ne, monkeypatch, name, xk, nbx, yk, nby, C, e
     y = _mi_operand(g, yk, B, nv, C, nby, base=x if (xk == 'q' and yk == 'q') else None)
     per_sm = int(env['NRT_MI_CTAS_PER_SM']) if 'NRT_MI_CTAS_PER_SM' in env else None
     _mi_case(ne, x, xk == 'q', nbx, y, yk == 'q', nby, B, C, nv, generic='NRT_MI_GENERIC' in env or nbx > 32,
-             per_sm=per_sm, env=env, tag='%s nv=%d' % (name, nv))
+             per_sm=per_sm, tag='%s nv=%d' % (name, nv))
 
 
 def test_mi_clip_constant_volume_and_explicit_centres_vs_fp64_reference(ne):
@@ -510,10 +507,8 @@ CONV_CASES = [
     ('col-K41', (1, 90, 8, 36, 1), 0, 41, 'SAME', 1, 1, {}),
     ('col4_64-even', (2, 20, 33, 12, 4), 1, 8, 'SAME', 1, 1, {}),
     ('col4_64-valid', (2, 70, 12, 40, 1), 0, 6, 'VALID', 1, 1, {}),
-    ('col4_32', (2, 70, 12, 40, 1), 0, 9, 'SAME', 1, 1, {'NRT_CONV_COL': '1'}),
-    ('col4_32-K41', (1, 90, 8, 36, 1), 1, 41, 'SAME', 1, 1, {'NRT_CONV_COL': '1'}),
-    ('col', (2, 70, 12, 40, 1), 0, 7, 'SAME', 1, 1, {'NRT_CONV_COL': '0'}),
-    ('col-even-K40', (1, 90, 8, 36, 1), 0, 40, 'SAME', 1, 1, {'NRT_CONV_COL': '0'}),
+    ('col', (2, 70, 11, 39, 1), 0, 7, 'SAME', 1, 1, {}),
+    ('col-even-K40', (1, 90, 8, 36, 1), 0, 40, 'SAME', 1, 1, {}),
     ('col-ragged', (2, 50, 33, 1), 0, 5, 'SAME', 1, 1, {}),
     ('row-inner1', (3, 300, 1), 0, 41, 'SAME', 1, 1, {}),
     ('row-inner1-even', (2, 9, 17, 70, 1), 2, 6, 'SAME', 1, 1, {}),
@@ -531,10 +526,10 @@ CONV_CASES = [
 
 @pytest.mark.parametrize('name,shape,axis,K,padding,stride,dil,env', CONV_CASES, ids=[c[0] for c in CONV_CASES])
 def test_sepconv_pass_vs_fp64_reference(ne, monkeypatch, name, shape, axis, K, padding, stride, dil, env):
-    """sepconv_col4_kernel<64> (default, K <= 32) and <32> (NRT_CONV_COL=1), sepconv_col_kernel (NRT_CONV_COL=0,
-    inner not a multiple of 4, K = 41 whose 64-row float4 tile would not fit 48 KB), sepconv_row_kernel (inner = 1,
-    2, 3, 17 < 32, and a dilated pass), sepconv_generic_kernel (stride, dilation on a column axis, VALID on a row,
-    NRT_CONV_GENERIC=1); K up to 41, even K under SAME, VALID; random kernels with cancellation."""
+    """sepconv_col4_kernel (K <= 32), sepconv_col_kernel (inner not a multiple of 4, K = 40 and 41 whose 64-row
+    float4 tile would not fit 48 KB), sepconv_row_kernel (inner = 1, 2, 3, 17 < 32, and a dilated pass),
+    sepconv_generic_kernel (stride, dilation on a column axis, VALID on a row, NRT_CONV_GENERIC=1); K up to 41, even K
+    under SAME, VALID; random kernels with cancellation."""
     for kv in env.items():
         monkeypatch.setenv(*kv)
     g = _g(sum(map(ord, name)))
@@ -561,7 +556,7 @@ def test_gaussian_blur_passes_vs_fp64_reference(ne):
 # =======================================================================================
 # dispatch
 # =======================================================================================
-def test_forward_dispatch_reaches_each_kernel(ne, monkeypatch):
+def test_forward_dispatch_launches_each_kernel(ne, monkeypatch):
     """The path tests above rely on the dispatch: record which kernels representative cases launch."""
     from torch.profiler import profile, ProfilerActivity
 
@@ -639,16 +634,16 @@ def test_forward_dispatch_reaches_each_kernel(ne, monkeypatch):
         cy = torch.linspace(0, 1, nby, device='cuda') if yk == 'q' else None
         generic = 'NRT_MI_GENERIC' in env or nbx > 32
         mt, nt = (1, 2) if max(nbx, nby) <= 16 else (2, 4)
-        minb = (3 if env.get('NRT_MI_VARIANT') in ('1', '2') and mt == 1 else 2) if xk == yk == 'q' else 1
+        minb = 2 if xk == yk == 'q' else 1
         want = 'mi_hist_generic_kernel' if generic else 'mi_hist_mma_kernel<%d,%d,%s,%s,%d,%d>' % (
-            mt, nt, str(xk == 'q').lower(), str(yk == 'q').lower(), _mi_spc(nbx, nby, xk == yk == 'q', env), minb)
+            mt, nt, str(xk == 'q').lower(), str(yk == 'q').lower(), _mi_spc(nbx, nby), minb)
         expect(lambda: _mi_hist(ne, xx, xk == 'q', nbx, cx, yy, yk == 'q', nby, cy, 2, C, 300, 30.0),
                [want, 'mi_combine_kernel'], env=env)
     # separable convolution
     for name, shape, axis, K, padding, stride, dil, env in CONV_CASES:
         x = torch.randn(shape, generator=g, device='cuda')
         kern = torch.randn(K, generator=g, device='cuda')
-        want = {'col4_64': 'sepconv_col4_kernel<64>', 'col4_32': 'sepconv_col4_kernel<32>', 'col': 'sepconv_col_kernel',
+        want = {'col4_64': 'sepconv_col4_kernel', 'col': 'sepconv_col_kernel',
                 'row': 'sepconv_row_kernel', 'generic': 'sepconv_generic_kernel'}[name.split('-')[0]]
         expect(lambda: ne.utils.separable_conv(x, [kern], axis=axis, batched=True, padding=padding, strides=stride,
                                                dilations=dil), [want], env=env)

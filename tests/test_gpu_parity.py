@@ -72,21 +72,23 @@ def test_spatial_transformer_golden(ne, name):
 
 
 # ------------------------------------------------------------------ tiled (TMA) path vs oracle
-def _rand_case(shape, amp, seed, smooth=False):
+def _rand_case(shape, amp, seed, smooth=False, channels=1):
     rng = np.random.default_rng(seed)
-    vol = rng.standard_normal((1,) + shape + (1,)).astype(F32)
+    vol = rng.standard_normal((1,) + shape + (channels,)).astype(F32)
     flow = rng.uniform(-amp, amp, (1,) + shape + (3,)).astype(F32)
     return vol, flow
 
 
-@pytest.mark.parametrize('cfg', [2, 3])
 @pytest.mark.parametrize('shape,amp,halo', [((20, 40, 64), 3.0, 3), ((17, 24, 36), 6.0, 4), ((9, 16, 32), 2.0, 5),
                                             ((33, 18, 100), 3.0, 0), ((40, 48, 96), 9.0, 8), ((16, 16, 36), 5.0, 4),
                                             ((12, 20, 32), 4.0, 4)])
 @pytest.mark.parametrize('method,fill', [('linear', None), ('linear', -2.5), ('nearest', 0.0)])
-def test_warp_tile_configs_bit_exact(ne, monkeypatch, cfg, shape, amp, halo, method, fill):
-    monkeypatch.setenv('NRT_WARP_TILE_CFG', str(cfg))
-    vol, flow = _rand_case(shape, amp, seed=cfg)
+@pytest.mark.parametrize('C', [1, 2])
+def test_warp_box_tile_bit_exact(ne, monkeypatch, C, shape, amp, halo, method, fill):
+    """TMA box-tile warp kernel: C = 1 on 8x8x32 tiles with the halo (3, 4, 6, 8) chosen from `halo`, C = 2 on
+    4x8x32 tiles with (x, channel) as one TMA dimension; flows inside, across and far outside the staged box; equal to
+    the oracle and to the generic gather kernel."""
+    vol, flow = _rand_case(shape, amp, seed=2, channels=C)
     flow[0, 0, 0, :4] = [[0, 0, 0], [0.5, 1.5, -0.5], [-40, 50, 3], [1, 1, 1]]
     ref = ointerp.spatial_transformer(vol, flow, method, 'ij', fill)
     lay = ne.layers.SpatialTransformer(interp_method=method, fill_value=fill, halo=halo)
@@ -101,9 +103,8 @@ def test_warp_tile_configs_bit_exact(ne, monkeypatch, cfg, shape, amp, halo, met
 @pytest.mark.parametrize('shape,amp', [((20, 24, 32), 3.0), ((11, 13, 52), 6.0), ((40, 18, 100), 2.5)])
 def test_warp_march_kernel_multichannel_bit_exact(ne, monkeypatch, C, shape, amp):
     """z-marching ring kernel (nrt_warp_march.cu): every channel count it is built for, ragged tiles, flows
-    inside and far outside the staged window, one / two / four quads per thread, forced z segmentations (down to one
-    output plane per segment)."""
-    monkeypatch.setenv('NRT_MARCH_SMALLC', '1')
+    inside and far outside the staged window, one and two quads per thread, forced z segmentations (down to one
+    output plane per segment); C = 2 takes the box-tile kernel."""
     rng = np.random.default_rng(C * 100 + shape[0])
     vol = rng.standard_normal((2,) + shape + (C,)).astype(F32)
     flow = rng.uniform(-amp, amp, (2,) + shape + (3,)).astype(F32)
@@ -115,10 +116,8 @@ def test_warp_march_kernel_multichannel_bit_exact(ne, monkeypatch, C, shape, amp
     for method, fill in (('linear', None), ('linear', -1.5), ('nearest', 0.0)):
         ref = ointerp.spatial_transformer(vol, flow, method, 'ij', fill)
         lay = ne.layers.SpatialTransformer(interp_method=method, fill_value=fill)
-        for env in ({}, {'NRT_MARCH_NW': '8', 'NRT_MARCH_QPT': '1'}, {'NRT_MARCH_NSEG': '3'},
-                    {'NRT_MARCH_QPT': '4'}, {'NRT_MARCH_NSEG': '40'}):
-            for k in ('NRT_MARCH_NW', 'NRT_MARCH_NSEG', 'NRT_MARCH_QPT'):
-                monkeypatch.delenv(k, raising=False)
+        for env in ({}, {'NRT_MARCH_NSEG': '3'}, {'NRT_MARCH_NSEG': '40'}):
+            monkeypatch.delenv('NRT_MARCH_NSEG', raising=False)
             for k, v in env.items():
                 monkeypatch.setenv(k, v)
             out = lay([dv, df]).cpu().numpy()
