@@ -275,6 +275,28 @@ NRT_API int nrt_sepconv_axis_f32(const float* x, float* out, int64_t outer, int6
 NRT_API int nrt_gather_axis_f32(const float* x, const int32_t* index, float* out, int64_t outer, int64_t L, int64_t inner,
                         int64_t L_out, void* stream);
 
+/* ---- noise fields: PerlinNoise / GaussianNoise (layers.py:2305-2508, augment.py:65-218) ----------------------
+ * A counter-based Philox4x32-10 stream: element i of a draw with `key` depends on (key, i) only (nrt_noise.cu
+ * documents the integer -> float conversion and the Box-Muller arithmetic).  Draws hold at most 2^31-1 elements.
+ * out[i] = lo + (hi - lo) * u_i, u_i in (0, 1]. */
+NRT_API int nrt_philox_uniform_f32(uint64_t key, int64_t n, float lo, float hi, float* out, void* stream);
+/* out[i] = z_i * sd[t(i)] * (*sd_scale if non-null) (+ x[i] if x is non-null), z_i standard normal.  shape[ndim]
+ * is the draw's row-major shape (ndim <= 5); the SD table sd has the row-major shape sd_shape[ndim], each extent
+ * equal to shape's or 1 (broadcast).  x may be null and must not alias out. */
+NRT_API int nrt_philox_normal_f32(uint64_t key, const int32_t* shape, const int32_t* sd_shape, int ndim, const float* sd,
+                          const float* sd_scale, const float* x, float* out, void* stream);
+/* Per-item statistics of x [items, n] in one pass: sums[item] = {sum d, sum d^2, max x, max |x|} (fp64,
+ * d = x - x[item, 0]; may be null) and stat[item] (fp32; may be null) = kind 0: population SD
+ * (tf.math.reduce_std), 1: max (reduce_max), 2: max |x|.  Deterministic: fixed-order block partials.
+ * workspace: nrt_item_stats_workspace_bytes(items, n). */
+NRT_API int64_t nrt_item_stats_workspace_bytes(int items, int64_t n);
+NRT_API int nrt_item_stats_f32(const float* x, int items, int64_t n, int kind, double* sums, float* stat, void* workspace,
+                       int64_t workspace_bytes, void* stream);
+/* Mean over Perlin levels: x [L, G, m] -> out [G, m],
+ *   out[g, i] = (sum_l x[l, g, i] * divide_no_nan(before[l*G + g], after[l*G + g])) / L   (levels in order). */
+NRT_API int nrt_level_combine_f32(const float* x, int L, int G, int64_t m, const float* before, const float* after,
+                          float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -14,6 +14,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'lib', 'libneurite_b200.so')
 
 c_i32, c_i64, c_f32, c_vp = ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_void_p
+c_u64 = ctypes.c_uint64
 P_I32 = ctypes.POINTER(ctypes.c_int32)
 
 # name -> (restype, argtypes); mirrors include/neurite_b200.h one to one
@@ -79,6 +80,11 @@ SIGNATURES = {
     'nrt_sepconv_axis_f32': (ctypes.c_int, [c_vp, c_vp, c_i64, c_i64, c_i64, c_vp, ctypes.c_int, ctypes.c_int,
                                              ctypes.c_int, ctypes.c_int, c_i64, c_vp]),
     'nrt_gather_axis_f32': (ctypes.c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_vp]),
+    'nrt_philox_uniform_f32': (ctypes.c_int, [c_u64, c_i64, c_f32, c_f32, c_vp, c_vp]),
+    'nrt_philox_normal_f32': (ctypes.c_int, [c_u64, P_I32, P_I32, ctypes.c_int, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    'nrt_item_stats_workspace_bytes': (c_i64, [ctypes.c_int, c_i64]),
+    'nrt_item_stats_f32': (ctypes.c_int, [c_vp, ctypes.c_int, c_i64, ctypes.c_int, c_vp, c_vp, c_vp, c_i64, c_vp]),
+    'nrt_level_combine_f32': (ctypes.c_int, [c_vp, ctypes.c_int, ctypes.c_int, c_i64, c_vp, c_vp, c_vp, c_vp]),
 }
 
 

@@ -6,6 +6,8 @@ neurite_b200.layers -- drop-ins for the hot-path layers of neurite.layers
     SpatialTransformer      voxelmorph.layers.SpatialTransformer (call sites models.py:806, 1157)
     VecInt, ComposeTransform, RescaleTransform   voxelmorph layers composed from the warp / resize
     LocallyConnected3D      layers.py:811-1197  (implementation 1)
+    GaussianBlur, Subsample layers.py:251-443
+    GaussianNoise, PerlinNoise   layers.py:2305-2508
 
 Constructor arguments, defaults, `get_config()` keys, `compute_output_shape`, weight names
 (`kernel`, `bias`) and weight shapes/orderings follow the reference, so configs and
@@ -17,7 +19,7 @@ import os
 import numpy as np
 import torch
 
-from . import _lib, utils
+from . import _lib, augment, utils
 from ._lib import lib, check, ptr, stream_ptr, i32_array, require_cuda
 
 
@@ -715,3 +717,155 @@ class Subsample(_Layer):
         self._calls += 1
         return utils.subsample_axis(x, stride_min=self.stride_min, stride_max=self.stride_max, axes=self.axes,
                                     prob=self.prob, upsample=self.upsample, seed=seed)
+
+
+# ---------------------------------------------------------------------------------------
+class _NoiseAddFn(torch.autograd.Function):
+    """x + noise in one pass (nrt_philox_normal_f32 reads x and writes the output); the noise does not depend
+    on x, so the gradient is the identity."""
+
+    @staticmethod
+    def forward(ctx, x32, key, shape_sd, table, scale):
+        out = torch.empty_like(x32)
+        with torch.cuda.device(x32.device):
+            check(lib.nrt_philox_normal_f32(key, i32_array(x32.shape), i32_array(shape_sd), x32.dim(), ptr(table),
+                                            ptr(scale), ptr(x32), ptr(out), stream_ptr(x32.device)))
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        return g, None, None, None, None
+
+
+class GaussianNoise(_Layer):
+    """Draw an SD from U[noise_min, noise_max] per index along `axes` and add N(0, SD) noise to the input, or
+    return the noise alone, reference layers.py:2305-2403.  With `absolute=False` the SD is relative to
+    max |x| over the whole tensor (computed on the device).  Randomness: see neurite_b200/augment.py; a layer
+    with a seed draws with `seed + number of earlier calls`."""
+
+    def __init__(self, noise_min=0.01, noise_max=0.10, noise_only=False, absolute=False, axes=(0, -1), seed=None,
+                 **kwargs):
+        self.noise_min = noise_min
+        self.noise_max = noise_max
+        self.noise_only = noise_only
+        self.absolute = absolute
+        self.axes = axes
+        self.seed = seed
+        self._calls = 0
+        super().__init__(**kwargs)
+
+    def get_config(self):
+        config = super().get_config().copy()
+        config.update({'noise_min': self.noise_min, 'noise_max': self.noise_max, 'noise_only': self.noise_only,
+                       'absolute': self.absolute, 'axes': self.axes, 'seed': self.seed})
+        return config
+
+    def build(self, input_shape):
+        num_dim = len(input_shape)
+        self.axes = np.ravel(self.axes)
+        self.axes = [int(ax) + num_dim if ax < 0 else int(ax) for ax in self.axes]
+        assert all(0 <= ax < num_dim for ax in self.axes), 'invalid axes'
+        super().build(input_shape)
+
+    def call(self, x):
+        if self.noise_max == 0 and not self.noise_only:
+            return x
+        if x.is_complex():
+            raise NotImplementedError('GaussianNoise: complex inputs are not supported')
+        assert x.dtype.is_floating_point, 'non-FP output type'
+        require_cuda(x)
+        if x.requires_grad and not self.absolute and torch.is_grad_enabled():
+            raise RuntimeError('GaussianNoise(absolute=False) has no gradient path through max|x|; '
+                               'pass a detached input or use absolute=True')
+        if not (np.isscalar(self.noise_min) and np.isscalar(self.noise_max)):
+            raise NotImplementedError('GaussianNoise: only scalar noise_min / noise_max are supported')
+        seed = None if self.seed is None else self.seed + self._calls
+        self._calls += 1
+        rand = np.random.default_rng(seed)
+        k_sd, k_noise = int(rand.integers(np.iinfo(int).max)), int(rand.integers(np.iinfo(int).max))
+
+        x32 = x if x.dtype == torch.float32 else x.to(torch.float32)
+        x32 = x32.contiguous()
+        shape_sd = [s if i in self.axes else 1 for i, s in enumerate(x32.shape)]
+        n_sd = int(np.prod(shape_sd, dtype=np.int64))
+        table = torch.empty(max(n_sd, 1), dtype=torch.float32, device=x.device)
+        scale = None
+        with torch.cuda.device(x.device):
+            st = stream_ptr(x.device)
+            check(lib.nrt_philox_uniform_f32(k_sd, n_sd, float(self.noise_min), float(self.noise_max), ptr(table),
+                                             st))
+            if not self.absolute and x32.numel():
+                scale = augment._item_stats(x32.detach().reshape(1, -1), 2)
+        if self.noise_only:
+            out = torch.empty_like(x32, memory_format=torch.contiguous_format)
+            with torch.cuda.device(x.device):
+                check(lib.nrt_philox_normal_f32(k_noise, i32_array(x32.shape), i32_array(shape_sd), x32.dim(),
+                                                ptr(table), ptr(scale), None, ptr(out), stream_ptr(x.device)))
+        else:
+            out = _NoiseAddFn.apply(x32, k_noise, shape_sd, table, scale)
+        return out.to(x.dtype) if x.dtype != torch.float32 else out
+
+    def compute_output_shape(self, input_shape):
+        return tuple(input_shape)
+
+
+class PerlinNoise(_Layer):
+    """Perlin noise drawn at full resolution for each batch item, reference layers.py:2406-2508: per level an
+    SD from U[noise_min, noise_max] (one per index along `axes`), N(0, SD) noise, a random Gaussian blur with
+    FWHMs in [fwhm_min, fwhm_max] that keeps `reduce` ('std', 'max' or a callable) constant, and the mean over
+    levels.  The input fixes the batch size (and the shape when `shape=None`).  Computed in fp32 and cast to
+    `out_type`.  Randomness: see neurite_b200/augment.py; a layer with a seed draws with
+    `seed + number of earlier calls`, and every item gets fresh draws."""
+
+    def __init__(self, shape=None, noise_min=0.01, noise_max=1, fwhm_min=4, fwhm_max=32, isotropic=False,
+                 reduce='std', out_type=torch.float32, axes=None, seed=None, **kwargs):
+        self.shape = shape
+        self.noise_min = noise_min
+        self.noise_max = noise_max
+        self.fwhm_min = fwhm_min
+        self.fwhm_max = fwhm_max
+        self.isotropic = isotropic
+        self.reduce = reduce
+        self.out_type = getattr(torch, out_type) if isinstance(out_type, str) else out_type
+        self.axes = axes
+        self.seed = seed
+        self._calls = 0
+        super().__init__(**kwargs)
+
+    def get_config(self):
+        config = super().get_config().copy()
+        config.update({'shape': self.shape, 'noise_min': self.noise_min, 'noise_max': self.noise_max,
+                       'fwhm_min': self.fwhm_min, 'fwhm_max': self.fwhm_max, 'isotropic': self.isotropic,
+                       'reduce': self.reduce, 'out_type': self.out_type, 'axes': self.axes, 'seed': self.seed})
+        return config
+
+    def build(self, input_shape):
+        allowed = range(1, len(input_shape))
+        self._axes = augment.normalize_axes(self.axes, input_shape, allowed, none_means_all=False)
+        super().build(input_shape)
+
+    def _plan(self, x, seed):
+        """(per-item level draws, item shape [1, *shape], SD-table shape) of one call with `seed`."""
+        fwhm_min, fwhm_max = augment._check_perlin_args(self.noise_min, self.noise_max, self.fwhm_min, self.fwhm_max)
+        shape = list(x.shape[1:]) if self.shape is None else [int(s) for s in self.shape]
+        gshape = [1] + shape                                   # draw_perlin_full(batched=False, featured=True)
+        shape_sd = [gshape[i] if i in self._axes else 1 for i in range(len(gshape))]
+        rand = np.random.default_rng(seed)
+        draws = [augment._level_draws(np.random.default_rng(int(rand.integers(np.iinfo(int).max))), len(shape) - 1,
+                                      fwhm_min, fwhm_max, self.isotropic) for _ in range(x.shape[0])]
+        return draws, gshape, shape_sd
+
+    def call(self, x):
+        require_cuda(x)
+        augment._stat_kind(self.reduce)
+        seed = None if self.seed is None else self.seed + self._calls
+        self._calls += 1
+        draws, gshape, shape_sd = self._plan(x, seed)
+        _, fwhm_max = augment._check_perlin_args(self.noise_min, self.noise_max, self.fwhm_min, self.fwhm_max)
+        out = augment._perlin(draws, gshape, shape_sd, self.noise_min, self.noise_max, fwhm_max, self.reduce,
+                              x.device)
+        out = out.reshape([x.shape[0]] + gshape[1:])
+        return out.to(self.out_type) if self.out_type != torch.float32 else out
+
+    def compute_output_shape(self, input_shape):
+        return (input_shape[0],) + tuple(input_shape[1:] if self.shape is None else self.shape)

@@ -682,3 +682,6 @@ def subsample_axis(x, stride_min=1, stride_max=8, axes=None, prob=1, upsample=Tr
     if prob < 1 and not (rand.uniform() < prob):
         thick = np.float32(1)
     return gather_axis(x, subsample_indices(x.shape[ax], thick, upsample), ax)
+
+
+from . import augment  # noqa: E402,F401  (ne.utils.augment.*, as in the reference)

@@ -31,8 +31,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
 import tfshim  # noqa: E402
 
-if len(sys.argv) != 2:
-    raise SystemExit('usage: python tools/gen_golden.py REFERENCE_ROOT')
+if len(sys.argv) < 2:
+    raise SystemExit('usage: python tools/gen_golden.py REFERENCE_ROOT [GROUP ...]')
 ne = tfshim.install(sys.argv[1])
 T = tfshim.Tensor
 OUT = os.path.join(os.path.dirname(HERE), 'tests', 'golden')
@@ -409,9 +409,63 @@ def gen_blur():
     save('sepconv_unbatched', ref, x=xs[0], k5=k5, k4=k4, out=out, kw=np.array('unbatched'))
 
 
+# ---------------------------------------------------------------------------------------
+# PerlinNoise / GaussianNoise / draw_perlin_full / random_blur_rescale  (augment.py:65-218, layers.py:2305-2508)
+# ---------------------------------------------------------------------------------------
+def gen_noise():
+    """The reference's own noise code on replayed draws: every tf.random call takes the next raw U[0, 1) or
+    N(0, 1) array from tfshim.REPLAY, whose log (q0, q1, ... in call order) is stored with the output."""
+    ref = ('reference neurite/tf/utils/augment.py:65-218 draw_perlin_full / random_blur_rescale, '
+           'layers.py:2305-2508 GaussianNoise / PerlinNoise on tfshim (tf.random replayed from the stored draws)')
+    tf = sys.modules['tensorflow']
+    rng = np.random.default_rng(90)
+    red = {'std': tf.math.reduce_std, 'max': tf.math.reduce_max}
+
+    def run(name, fn, **meta):
+        tfshim.REPLAY = tfshim.Replay(rng)
+        out = npy(fn())
+        q = {'q%d' % i: d for i, d in enumerate(tfshim.REPLAY.log)}
+        save(name, ref, out=out, nq=np.array(len(q)), **q, **{k: np.asarray(v) for k, v in meta.items()})
+
+    cases = [  # name, shape, levels (fwhm_min, fwhm_max), isotropic, reduce, axes, batched, featured
+        ('perlin_2d_l1_std', (23, 31), ([2], [6]), False, 'std', None, False, False),
+        ('perlin_2d_l3_max_iso', (20, 17, 2), ([1, 3, 5], [2, 8, 12]), True, 'max', -1, False, True),
+        ('perlin_3d_l2_std_ax', (9, 12, 14, 3), ([2, 4], [4, 9]), False, 'std', -1, False, True),
+        ('perlin_3d_l1_max_b2', (2, 10, 11, 13, 1), ([3], [7]), True, 'max', None, True, True),
+        ('perlin_3d_l2_std_iso', (8, 9, 10), ([1, 2], [3, 5]), True, 'std', None, False, False),
+    ]
+    for name, shape, (lo, hi), iso, rd, axes, batched, featured in cases:
+        run(name, lambda: ne.utils.augment.draw_perlin_full(
+            list(shape), noise_min=0.05, noise_max=1.5, fwhm_min=lo, fwhm_max=hi, isotropic=iso, batched=batched,
+            featured=featured, reduce=red[rd], axes=axes), shape=shape, fwhm_min=lo, fwhm_max=hi, isotropic=iso,
+            reduce=rd, axes=-9 if axes is None else axes, batched=batched, featured=featured, noise_min=0.05,
+            noise_max=1.5)
+
+    x = rng.standard_normal((2, 12, 14, 3)).astype(F32)
+    run('perlin_layer_2d_l2_std', lambda: ne.layers.PerlinNoise(fwhm_min=[2, 3], fwhm_max=[4, 6], axes=-1)(T(x)),
+        x=x, fwhm_min=[2, 3], fwhm_max=[4, 6], isotropic=False, reduce='std', axes=-1, noise_min=0.01, noise_max=1.0)
+    x3 = rng.standard_normal((2, 7, 9, 11, 1)).astype(F32)
+    run('perlin_layer_3d_l1_max', lambda: ne.layers.PerlinNoise(shape=(7, 9, 11, 2), fwhm_min=3, fwhm_max=8,
+                                                                   isotropic=True, reduce=tf.math.reduce_max)(T(x3)),
+        x=x3, shape=(7, 9, 11, 2), fwhm_min=[3], fwhm_max=[8], isotropic=True, reduce='max', axes=-9,
+        noise_min=0.01, noise_max=1.0)
+    xb = rng.standard_normal((1, 15, 16, 2)).astype(F32)
+    run('perlin_blur_rescale_2d_std', lambda: ne.utils.augment.random_blur_rescale(T(xb), std_min=0.5, std_max=2.5,
+                                                                              batched=True),
+        x=xb, std_min=0.5, std_max=2.5, isotropic=False, reduce='std')
+
+    xg = (3 * rng.standard_normal((2, 6, 7, 8, 3))).astype(F32)
+    for tag, kw in (('default', {}), ('noise_only', dict(noise_only=True)), ('absolute', dict(absolute=True)),
+                    ('abs_only_ax1', dict(absolute=True, noise_only=True, axes=1))):
+        kw = dict(noise_min=0.1, noise_max=0.2, **kw)
+        run('gaussnoise_' + tag, lambda: ne.layers.GaussianNoise(**kw)(T(xg)), x=xg,
+            **{k: v for k, v in kw.items()})
+
+
 if __name__ == '__main__':
-    only = sys.argv[1:]
-    for fn in (gen_interpn, gen_resize, gen_spatial_transformer, gen_dice, gen_lc3d, gen_lc3d_impl, gen_mi, gen_blur):
+    only = sys.argv[2:]
+    for fn in (gen_interpn, gen_resize, gen_spatial_transformer, gen_dice, gen_lc3d, gen_lc3d_impl, gen_mi, gen_blur,
+               gen_noise):
         if not only or fn.__name__[4:] in only:
             fn()
     tot = sum(os.path.getsize(os.path.join(OUT, f)) for f in os.listdir(OUT))

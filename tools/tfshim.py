@@ -61,6 +61,14 @@ class DType:
         return np.issubdtype(self.np, np.integer)
 
     @property
+    def is_complex(self):
+        return np.issubdtype(self.np, np.complexfloating)
+
+    @property
+    def real_dtype(self):
+        return self
+
+    @property
     def base_dtype(self):
         return self
 
@@ -179,6 +187,7 @@ class Tensor:
     def __truediv__(self, o): return self._bin(o, np.true_divide)
     def __rtruediv__(self, o): return self._bin(o, np.true_divide, True)
     def __neg__(self): return Tensor(-self._a)
+    def __pow__(self, o): return self._bin(o, np.power)
     def __lt__(self, o): return self._bin(o, np.less)
     def __le__(self, o): return self._bin(o, np.less_equal)
     def __gt__(self, o): return self._bin(o, np.greater)
@@ -255,6 +264,76 @@ class _Finder(importlib.abc.MetaPathFinder, importlib.abc.Loader):
     def exec_module(self, module):
         if module.__name__ == 'pystrum':
             module.__version__ = '0.4'
+
+
+# ---------------------------------------------------------------------------------------
+# replayed randomness
+# ---------------------------------------------------------------------------------------
+class Replay:
+    """The raw draws behind tf.random.uniform / tf.random.normal and tf.random.Generator, in call order.
+
+    Each call takes the next raw array of the call's shape -- from the queue given to `feed`, else from the
+    numpy generator `rng` -- and appends it to `log`: U[0, 1) for uniform, N(0, 1) for normal, fp32.  TF's fp32
+    arithmetic on top is applied by the ops: uniform `u * (maxval - minval) + minval`, normal
+    `z * stddev + mean`.  A fixture stores `log`; replaying it reproduces the call."""
+
+    def __init__(self, rng=None):
+        self.rng = rng if rng is not None else np.random.default_rng(0)
+        self.queue = []
+        self.log = []
+
+    def feed(self, draws):
+        self.queue = [np.asarray(d, np.float32) for d in draws]
+
+    def take(self, kind, shape):
+        shape = tuple(int(v) for v in np.ravel(A(T(shape))))
+        if self.queue:
+            raw = self.queue.pop(0)
+            assert raw.shape == shape, 'replayed draw of shape %s, call wants %s' % (raw.shape, shape)
+        elif kind == 'uniform':
+            raw = self.rng.random(shape, dtype=np.float32)
+        else:
+            raw = self.rng.standard_normal(shape, dtype=np.float32)
+        self.log.append(raw)
+        return raw
+
+
+REPLAY = Replay()
+
+
+def _uniform(shape, minval=0, maxval=None, dtype=None, seed=None, **k):
+    dt = np.float32 if dtype is None else _np_dtype(dtype)
+    lo = np.asarray(A(T(minval)), dt)
+    hi = np.asarray(A(T(1 if maxval is None else maxval)), dt)
+    u = REPLAY.take('uniform', shape).astype(dt)
+    return Tensor((u * (hi - lo) + lo).astype(dt))
+
+
+def _normal(shape, mean=0.0, stddev=1.0, dtype=None, seed=None, **k):
+    dt = np.float32 if dtype is None else _np_dtype(dtype)
+    z = REPLAY.take('normal', shape).astype(dt)
+    return Tensor((z * np.asarray(A(T(stddev)), dt) + np.asarray(A(T(mean)), dt)).astype(dt))
+
+
+class _Generator:
+    """tf.random.Generator on the replayed stream (the state and seed do not select the values)."""
+
+    @classmethod
+    def from_non_deterministic_state(cls):
+        return cls()
+
+    @classmethod
+    def from_seed(cls, seed, **k):
+        return cls()
+
+    def reset_from_seed(self, seed):
+        pass
+
+    def uniform(self, shape, minval=0, maxval=None, dtype=None, **k):
+        return _uniform(shape, minval, maxval, dtype)
+
+    def normal(self, shape, mean=0.0, stddev=1.0, dtype=None, **k):
+        return _normal(shape, mean, stddev, dtype)
 
 
 # ---------------------------------------------------------------------------------------
@@ -370,7 +449,21 @@ def _install_tf():
         np.divide(a, b, out=out, where=(b != 0))
         return Tensor(out)
     tfmath.divide_no_nan = divide_no_nan
+    # reductions over the whole tensor: float64, one rounding (TF's order is unspecified); reduce_std is the
+    # population SD
+    tfmath.reduce_std = lambda x, axis=None, keepdims=False: Tensor(
+        np.std(A(T(x)).astype(np.float64), axis=axis, keepdims=keepdims).astype(A(T(x)).dtype))
+    tfmath.reduce_max = lambda x, axis=None, keepdims=False: Tensor(np.max(A(T(x)), axis=axis, keepdims=keepdims))
+    tf.reduce_max = tfmath.reduce_max
+    tf.abs = lambda x: Tensor(np.abs(A(T(x))))
+    tfmath.abs = tf.abs
     tf.math = tfmath
+
+    rnd = _InertModule('tensorflow.random')
+    rnd.uniform = _uniform
+    rnd.normal = _normal
+    rnd.Generator = _Generator
+    tf.random = rnd
 
     class InvalidArgumentError(Exception):
         pass
@@ -496,7 +589,7 @@ def _install_tf():
         'tensorflow.keras': keras, 'tensorflow.keras.backend': K,
         'tensorflow.keras.layers': layers, 'tensorflow.keras.losses': losses,
         'tensorflow.nn': nn, 'tensorflow.dtypes': dtypes, 'tensorflow.experimental': exp_mod,
-        'tensorflow.experimental.numpy': exp_np,
+        'tensorflow.experimental.numpy': exp_np, 'tensorflow.random': rnd,
     }
     sys.modules.update(mods)
 
