@@ -296,6 +296,51 @@ NRT_API int nrt_item_stats_f32(const float* x, int items, int64_t n, int kind, d
  *   out[g, i] = (sum_l x[l, g, i] * divide_no_nan(before[l*G + g], after[l*G + g])) / L   (levels in order). */
 NRT_API int nrt_level_combine_f32(const float* x, int L, int G, int64_t m, const float* before, const float* after,
                           float* out, void* stream);
+/* GaussianNoise fused with the generator's background clearing (models.py:1219-1231), x and out [B, V, C]:
+ *   out[i] = (x[i] + z_i * (sd[b * C + c] * *sd_scale)) * (label(b, v) == 0 && bg_u[b] < zero_background ? 0 : 1)
+ * with z_i the normals of nrt_philox_normal_f32 for the same key and shape [B, V, C], bit for bit.  label(b, v) is
+ * int32(labels[b * V + v]) inside the crop window of nrt_labels_to_image_f32, 0 outside. */
+NRT_API int nrt_philox_normal_background_f32(uint64_t key, int B, int64_t V, int C, const float* sd,
+                          const float* sd_scale, const float* x, const float* labels, int64_t crop_L,
+                          int64_t crop_inner, int64_t crop_lo, int64_t crop_hi, const float* bg_u,
+                          float zero_background, float* out, void* stream);
+
+/* ---- label-to-image synthesis: labels_to_image_new (models.py:1162-1282), RandomCrop (layers.py:446-519) ------
+ * labels [B, V] fp32 holds the warped label map; a voxel's label is int32(trunc(x)).  The crop window keeps the
+ * voxels v with (v / crop_inner) % crop_L in [crop_lo, crop_hi) and sets the others' label to 0; (1, 1, 0, 1)
+ * keeps all.  A LUT lookup outside [0, nlut) gives 0 (TF's GPU gather).
+ * Image: idx = gen_lut[label]; mean = u[b, c, idx] * (mean_max[c, idx] - mean_min[c, idx]) + mean_min[c, idx]
+ * (mean_min / mean_max [C, N]);
+ * image[b, v, c] = mean (* f, f = bias[b, v, c], expf'd when apply_exp), each op rounded once.  mean_out and
+ * bias_out (may be null; need bias) receive mean and f.  *absmax = max |image| over the whole batch (device
+ * scalar, deterministic).  workspace: nrt_labels_to_image_workspace_bytes(). */
+NRT_API int64_t nrt_labels_to_image_workspace_bytes(void);
+NRT_API int nrt_labels_to_image_f32(const float* labels, int B, int64_t V, int C, int64_t crop_L, int64_t crop_inner,
+                          int64_t crop_lo, int64_t crop_hi, const int32_t* gen_lut, int nlut, int N,
+                          const float* u, const float* mean_min, const float* mean_max, const float* bias,
+                          int apply_exp, float* image, float* mean_out, float* bias_out, float* absmax,
+                          void* workspace, int64_t workspace_bytes, void* stream);
+/* Per-item min and max of x [items, n]: mnmx[2 * item] = min, mnmx[2 * item + 1] = max (fixed-order block
+ * partials).  workspace: nrt_item_minmax_workspace_bytes(items, n). */
+NRT_API int64_t nrt_item_minmax_workspace_bytes(int items, int64_t n);
+NRT_API int nrt_item_minmax_f32(const float* x, int items, int64_t n, float* mnmx, void* workspace,
+                          int64_t workspace_bytes, void* stream);
+/* x [items, n] with n = V * C -> out: y = x; with mnmx, y = div_no_nan(y - mn, mx - mn); with gamma_u [items, C],
+ * y = powf(y, gamma_u[item, c] * (gamma_hi - gamma_lo) + gamma_lo).  out must not alias x. */
+NRT_API int nrt_norm_gamma_f32(const float* x, int items, int64_t n, int C, const float* mnmx, const float* gamma_u,
+                          float gamma_lo, float gamma_hi, float* out, void* stream);
+/* Output label map: l = crop(label), then l = lut[l] when lut is non-null.  _f32 writes the one-hot out [B, V, M]
+ * (all-zero row when l is outside [0, M)); _i32 writes l to out [B, V]. */
+NRT_API int nrt_label_map_f32(const float* labels, int B, int64_t V, int64_t crop_L, int64_t crop_inner,
+                          int64_t crop_lo, int64_t crop_hi, const int32_t* lut, int nlut, int M, float* out,
+                          void* stream);
+NRT_API int nrt_label_map_i32(const float* labels, int B, int64_t V, int64_t crop_L, int64_t crop_inner,
+                          int64_t crop_lo, int64_t crop_hi, const int32_t* lut, int nlut, int32_t* out, void* stream);
+/* out[o, l, i] = x[o, l, i] * (lo <= l < hi) on [outer, L, inner] (RandomCrop's mask); out must not alias x. */
+NRT_API int nrt_crop_window_f32(const float* x, int64_t outer, int64_t L, int64_t inner, int64_t lo, int64_t hi,
+                          float* out, void* stream);
+NRT_API int nrt_crop_window_i32(const int32_t* x, int64_t outer, int64_t L, int64_t inner, int64_t lo, int64_t hi,
+                          int32_t* out, void* stream);
 
 #ifdef __cplusplus
 }

@@ -17,5 +17,5 @@ fails if that library has not been built -- there is no CPU fallback.
 __version__ = '0.1'
 
 from . import _lib  # noqa: F401  (raises ImportError when the CUDA library is missing)
-from . import utils, layers, metrics, losses, dist  # noqa: F401
+from . import utils, layers, metrics, losses, dist, models, augment  # noqa: F401
 from .utils import interpn, resize, zoom, transform  # noqa: F401

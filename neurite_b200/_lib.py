@@ -85,6 +85,22 @@ SIGNATURES = {
     'nrt_item_stats_workspace_bytes': (c_i64, [ctypes.c_int, c_i64]),
     'nrt_item_stats_f32': (ctypes.c_int, [c_vp, ctypes.c_int, c_i64, ctypes.c_int, c_vp, c_vp, c_vp, c_i64, c_vp]),
     'nrt_level_combine_f32': (ctypes.c_int, [c_vp, ctypes.c_int, ctypes.c_int, c_i64, c_vp, c_vp, c_vp, c_vp]),
+    'nrt_philox_normal_background_f32': (ctypes.c_int, [c_u64, ctypes.c_int, c_i64, ctypes.c_int, c_vp, c_vp, c_vp,
+                                                         c_vp, c_i64, c_i64, c_i64, c_i64, c_vp, c_f32, c_vp, c_vp]),
+    'nrt_labels_to_image_workspace_bytes': (c_i64, []),
+    'nrt_labels_to_image_f32': (ctypes.c_int, [c_vp, ctypes.c_int, c_i64, ctypes.c_int, c_i64, c_i64, c_i64, c_i64,
+                                                c_vp, ctypes.c_int, ctypes.c_int, c_vp, c_vp, c_vp, c_vp, ctypes.c_int,
+                                                c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]),
+    'nrt_item_minmax_workspace_bytes': (c_i64, [ctypes.c_int, c_i64]),
+    'nrt_item_minmax_f32': (ctypes.c_int, [c_vp, ctypes.c_int, c_i64, c_vp, c_vp, c_i64, c_vp]),
+    'nrt_norm_gamma_f32': (ctypes.c_int, [c_vp, ctypes.c_int, c_i64, ctypes.c_int, c_vp, c_vp, c_f32, c_f32, c_vp,
+                                           c_vp]),
+    'nrt_label_map_f32': (ctypes.c_int, [c_vp, ctypes.c_int, c_i64, c_i64, c_i64, c_i64, c_i64, c_vp, ctypes.c_int,
+                                          ctypes.c_int, c_vp, c_vp]),
+    'nrt_label_map_i32': (ctypes.c_int, [c_vp, ctypes.c_int, c_i64, c_i64, c_i64, c_i64, c_i64, c_vp, ctypes.c_int,
+                                          c_vp, c_vp]),
+    'nrt_crop_window_f32': (ctypes.c_int, [c_vp, c_i64, c_i64, c_i64, c_i64, c_i64, c_vp, c_vp]),
+    'nrt_crop_window_i32': (ctypes.c_int, [c_vp, c_i64, c_i64, c_i64, c_i64, c_i64, c_vp, c_vp]),
 }
 
 

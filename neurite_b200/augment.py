@@ -4,6 +4,7 @@ neurite_b200.augment -- the noise fields of neurite's synthesis generator
 
     random_blur_rescale(x, std_min, std_max, isotropic, seed, reduce, batched)   augment.py:65-112
     draw_perlin_full(shape, noise_min, noise_max, fwhm_min, fwhm_max, ...)      augment.py:115-218
+    draw_crop_mask(x, crop_min, crop_max, axis, prob, bilateral, seed)          augment.py:221-287
 
 Also reachable as `neurite_b200.utils.augment`, as in the reference.
 
@@ -219,6 +220,80 @@ def random_blur_rescale(x, std_min=8 / 2.355, std_max=32 / 2.355, isotropic=Fals
     out = _draw_perlin_full_from_draws(xb[None, None], [[sig]], [std_max], reduce)[0]
     out = out if batched else out[0]
     return out.to(x.dtype) if x.dtype != torch.float32 else out
+
+
+def tf_range_f32(width):
+    """tf.range(1, delta=1 / width) in fp32 (provenance: contract; TF's RangeOp, restated): delta = 1 / width,
+    length ceil(1 / delta) and element i = i * delta, each op rounded once in fp32."""
+    f32 = np.float32
+    delta = f32(f32(1) / f32(width))
+    n = int(np.ceil(f32(f32(1) / delta)))
+    return (np.arange(n, dtype=f32) * delta).astype(f32)
+
+
+def crop_bounds(width, prop_low, prop_cen):
+    """The index range [lo, hi) where draw_crop_mask's mask is 1 (augment.py:280-284): prop >= prop_low and
+    prop < prop_low + prop_cen in fp32 on prop = tf.range(1, delta=1/width).  prop is non-decreasing, so the mask
+    is one contiguous range.  ValueError where the range's length is not `width` (the reference's reshape
+    fails there)."""
+    f32 = np.float32
+    prop = tf_range_f32(width)
+    if prop.size != width:
+        raise ValueError(f'tf.range(1, delta=1/{width}) has {prop.size} elements, not {width}: cannot reshape the '
+                         f'crop mask')
+    pl = f32(prop_low)
+    ph = f32(pl + f32(prop_cen))
+    lo = int(np.searchsorted(prop, pl, side='left'))
+    hi = int(np.searchsorted(prop, ph, side='left'))
+    return lo, max(lo, hi)
+
+
+def _draw_crop(shape, crop_min, crop_max, axis, prob, bilateral, seed):
+    """draw_crop_mask's draws (augment.py:246-277) on the host -> (axis, lo, hi).  Each of the reference's
+    tf.random.uniform calls takes the next integer of a numpy generator seeded with `seed`, and draws from a
+    numpy generator seeded with that integer; the fp32 arithmetic on the draws is TF's."""
+    f32 = np.float32
+    rand = np.random.default_rng(seed)
+
+    def gen():
+        return np.random.default_rng(int(rand.integers(_MAX_SEED)))
+
+    axis = normalize_axes(axis, shape, none_means_all=True)
+    assert 0 <= crop_min <= crop_max <= 1, f'invalid proportions {crop_min}, {crop_max}'
+    prop_cut = f32(crop_max)
+    if crop_min < crop_max:
+        lo_, hi_ = f32(crop_min), f32(crop_max)
+        prop_cut = f32(f32(gen().random(dtype=f32) * f32(hi_ - lo_)) + lo_)
+    assert 0 <= prob <= 1, f'{prob} not a probability'
+    if prob < 1:
+        bit = gen().random(dtype=f32) < f32(prob)
+        prop_cut = f32(prop_cut * f32(bit))
+    rand_prop = gen().random(dtype=f32)
+    if not bilateral:
+        rand_prop = f32(rand_prop < f32(0.5))
+    prop_low = f32(prop_cut * rand_prop)
+    prop_cen = f32(f32(1) - prop_cut)
+    ax = axis[int(gen().integers(len(axis)))]
+    lo, hi = crop_bounds(int(shape[ax]), prop_low, prop_cen)
+    return ax, lo, hi
+
+
+def draw_crop_mask(x, crop_min=0, crop_max=0.5, axis=None, prob=1, bilateral=False, seed=None):
+    """Mask that crops the field of view of x along one axis (augment.py:221-287): 1 on a drawn index range
+    [lo, hi) of one drawn axis, 0 elsewhere, with the shape (1, .., width, .., 1) and x's dtype.  A torch
+    tensor on x's device for a tensor x, else a numpy array.  The draws are made on the host (_draw_crop)."""
+    if isinstance(x, (list, tuple)):
+        x = torch.cat(list(x), 0) if torch.is_tensor(x[0]) else np.concatenate(x, 0)
+    shape = list(x.shape)
+    ax, lo, hi = _draw_crop(shape, crop_min, crop_max, axis, prob, bilateral, seed)
+    mshape = [1] * len(shape)
+    mshape[ax] = shape[ax]
+    mask = np.zeros(shape[ax], np.float32)
+    mask[lo:hi] = 1
+    mask = mask.reshape(mshape)
+    if torch.is_tensor(x):
+        return torch.as_tensor(mask, device=x.device).to(x.dtype)
+    return mask.astype(np.asarray(x).dtype)
 
 
 def draw_perlin_full(shape, noise_min=0.01, noise_max=1, fwhm_min=4, fwhm_max=32, isotropic=False, batched=False,

@@ -75,6 +75,17 @@ __global__ void __launch_bounds__(256) philox_uniform_kernel(uint32_t k0, uint32
   }
 }
 
+// the four standard normals of block j (Box-Muller on the word pairs)
+__device__ __forceinline__ void philox_normal4(uint32_t j, uint32_t k0, uint32_t k1, float z[4]) {
+  const uint4 w = philox4x32_10(j, 0u, k0, k1);
+  const float r0 = sqrtf(-2.f * logf(u01(w.x))), r1 = sqrtf(-2.f * logf(u01(w.z)));
+  float s0, c0, s1, c1;
+  sincospif(2.f * u01(w.y), &s0, &c0);
+  sincospif(2.f * u01(w.w), &s1, &c1);
+  z[0] = __fmul_rn(r0, c0); z[1] = __fmul_rn(r0, s0);
+  z[2] = __fmul_rn(r1, c1); z[3] = __fmul_rn(r1, s1);
+}
+
 __global__ void __launch_bounds__(256) philox_normal_kernel(uint32_t k0, uint32_t k1, uint32_t n, const Bcast b,
                                                             const float* __restrict__ sd,
                                                             const float* __restrict__ scale,
@@ -82,16 +93,8 @@ __global__ void __launch_bounds__(256) philox_normal_kernel(uint32_t k0, uint32_
                                                             int vec) {
   const uint32_t j = blockIdx.x * 256u + threadIdx.x;
   if ((uint64_t)j * 4 >= n) return;
-  const uint4 w = philox4x32_10(j, 0u, k0, k1);
   float z[4];
-  {
-    const float r0 = sqrtf(-2.f * logf(u01(w.x))), r1 = sqrtf(-2.f * logf(u01(w.z)));
-    float s0, c0, s1, c1;
-    sincospif(2.f * u01(w.y), &s0, &c0);
-    sincospif(2.f * u01(w.w), &s1, &c1);
-    z[0] = __fmul_rn(r0, c0); z[1] = __fmul_rn(r0, s0);
-    z[2] = __fmul_rn(r1, c1); z[3] = __fmul_rn(r1, s1);
-  }
+  philox_normal4(j, k0, k1, z);
   const float sc = scale ? __ldg(scale) : 1.f;
   const uint32_t i0 = j * 4u;
   float v[4];
@@ -114,6 +117,34 @@ __global__ void __launch_bounds__(256) philox_normal_kernel(uint32_t k0, uint32_
   for (int q = 0; q < 4; ++q) {
     const uint32_t i = i0 + q;
     if (i < n) out[i] = x ? __fadd_rn(x[i], v[q]) : v[q];
+  }
+}
+
+// GaussianNoise of the generator fused with its background clearing (models.py:1219-1231) on x [B, V, C]:
+// out[i] = (x[i] + z_i * (sd[b, c] * scale)) * keep, keep = 0 where label(b, v) == 0 and bg_u[b] < zb, else 1.
+// z_i is element i of the same draw as philox_normal_kernel with shape [B, V, C] and the SD table [B, 1, C].
+// label(b, v) = int32(labels[b, v]) inside the crop window (v / crop_inner) % crop_L in [crop_lo, crop_hi), else 0.
+__global__ void __launch_bounds__(256) philox_normal_background_kernel(
+    uint32_t k0, uint32_t k1, uint32_t V, uint32_t C, uint32_t n, const float* __restrict__ sd,
+    const float* __restrict__ scale, const float* __restrict__ x, const float* __restrict__ labels, uint32_t crop_L,
+    uint32_t crop_inner, uint32_t crop_lo, uint32_t crop_hi, const float* __restrict__ bg_u, float zb,
+    float* __restrict__ out) {
+  const uint32_t j = blockIdx.x * 256u + threadIdx.x;
+  if ((uint64_t)j * 4 >= n) return;
+  float z[4];
+  philox_normal4(j, k0, k1, z);
+  const float sc = __ldg(scale);
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const uint32_t i = j * 4u + q;
+    if (i >= n) break;
+    const uint32_t bv = i / C, c = i - bv * C, b = bv / V, v = bv - b * V;
+    const float s = __fmul_rn(__ldg(sd + b * C + c), sc);
+    const float y = __fadd_rn(x[i], __fmul_rn(z[q], s));
+    const uint32_t a = (v / crop_inner) % crop_L;
+    const int lab = (a >= crop_lo && a < crop_hi) ? __float2int_rz(__ldg(labels + bv)) : 0;
+    const bool clear = lab == 0 && __ldg(bg_u + b) < zb;
+    out[i] = __fmul_rn(y, clear ? 0.f : 1.f);
   }
 }
 
@@ -278,6 +309,24 @@ int nrt_philox_normal_f32(uint64_t key, const int32_t* shape, const int32_t* sd_
   philox_normal_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(
       (uint32_t)key, (uint32_t)(key >> 32), (uint32_t)n, b, sd, sd_scale, x, out, vec);
   return check_launch("philox_normal_kernel");
+}
+
+int nrt_philox_normal_background_f32(uint64_t key, int B, int64_t V, int C, const float* sd, const float* sd_scale,
+                                     const float* x, const float* labels, int64_t crop_L, int64_t crop_inner,
+                                     int64_t crop_lo, int64_t crop_hi, const float* bg_u, float zero_background,
+                                     float* out, void* stream) {
+  NRT_REQUIRE(sd && sd_scale && x && labels && bg_u && out, NRT_E_ARG, "null pointer");
+  NRT_REQUIRE(x != out, NRT_E_ARG, "in-place noise is not supported");
+  NRT_REQUIRE(B >= 1 && V >= 1 && C >= 1, NRT_E_ARG, "bad B / V / C");
+  NRT_REQUIRE(crop_L >= 1 && crop_inner >= 1 && V % (crop_L * crop_inner) == 0 && crop_lo >= 0 && crop_lo <= crop_hi &&
+                  crop_hi <= crop_L, NRT_E_ARG, "bad crop window");
+  const int64_t n = (int64_t)B * V * C;
+  NRT_REQUIRE(n <= 2147483647LL, NRT_E_SIZE, "draw of %lld elements > 2^31-1", (long long)n);
+  const unsigned blocks = (unsigned)((n + 1023) / 1024);
+  philox_normal_background_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      (uint32_t)key, (uint32_t)(key >> 32), (uint32_t)V, (uint32_t)C, (uint32_t)n, sd, sd_scale, x, labels,
+      (uint32_t)crop_L, (uint32_t)crop_inner, (uint32_t)crop_lo, (uint32_t)crop_hi, bg_u, zero_background, out);
+  return check_launch("philox_normal_background_kernel");
 }
 
 int64_t nrt_item_stats_workspace_bytes(int items, int64_t n) {

@@ -7,6 +7,7 @@ neurite_b200.layers -- drop-ins for the hot-path layers of neurite.layers
     VecInt, ComposeTransform, RescaleTransform   voxelmorph layers composed from the warp / resize
     LocallyConnected3D      layers.py:811-1197  (implementation 1)
     GaussianBlur, Subsample layers.py:251-443
+    RandomCrop              layers.py:446-519
     GaussianNoise, PerlinNoise   layers.py:2305-2508
 
 Constructor arguments, defaults, `get_config()` keys, `compute_output_shape`, weight names
@@ -717,6 +718,77 @@ class Subsample(_Layer):
         self._calls += 1
         return utils.subsample_axis(x, stride_min=self.stride_min, stride_max=self.stride_max, axes=self.axes,
                                     prob=self.prob, upsample=self.upsample, seed=seed)
+
+
+def _crop_window(x, axis, lo, hi):
+    """x * mask with mask 1 on [lo, hi) along `axis` (nrt_crop_window_{f32,i32}); fp32 or int32 x."""
+    shp = list(x.shape)
+    outer = int(np.prod(shp[:axis], dtype=np.int64))
+    inner = int(np.prod(shp[axis + 1:], dtype=np.int64))
+    out = torch.empty_like(x, memory_format=torch.contiguous_format)
+    fn = lib.nrt_crop_window_f32 if x.dtype == torch.float32 else lib.nrt_crop_window_i32
+    with torch.cuda.device(x.device):
+        check(fn(ptr(x), outer, shp[axis], inner, int(lo), int(hi), ptr(out), stream_ptr(x.device)))
+    return out
+
+
+class _CropFn(torch.autograd.Function):
+    """x * mask; the gradient is the upstream gradient times the same mask."""
+
+    @staticmethod
+    def forward(ctx, x, axis, lo, hi):
+        ctx.window = (axis, lo, hi)
+        return _crop_window(x.contiguous(), axis, lo, hi)
+
+    @staticmethod
+    def backward(ctx, g):
+        return _crop_window(g.to(torch.float32).contiguous(), *ctx.window), None, None, None
+
+
+class RandomCrop(_Layer):
+    """Crop the content of a tensor [B, *space, C] by multiplying with a binary mask that is 1 on a random index
+    range of one random spatial axis, reference layers.py:446-519 with augment.draw_crop_mask.  fp32 or int32
+    input.  Randomness: see neurite_b200/augment.py; a layer with a seed draws with `seed + number of earlier
+    calls`.  The mask is applied by nrt_crop_window_{f32,i32}; the gradient is the same mask."""
+
+    def __init__(self, crop_min=0, crop_max=0.5, axis=None, prob=1, bilateral=False, seed=None, **kwargs):
+        self.crop_min = crop_min
+        self.crop_max = crop_max
+        self.axis = axis
+        self.prob = prob
+        self.bilateral = bilateral
+        self.seed = seed
+        self._calls = 0
+        super().__init__(**kwargs)
+
+    def get_config(self):
+        config = super().get_config().copy()
+        config.update({'crop_min': self.crop_min, 'crop_max': self.crop_max, 'axis': self.axis, 'prob': self.prob,
+                       'bilateral': self.bilateral, 'seed': self.seed})
+        return config
+
+    def build(self, input_shape):
+        ndims = len(input_shape) - 2
+        self.axis = augment.normalize_axes(self.axis, input_shape, range(1, ndims + 1), none_means_all=True)
+        super().build(input_shape)
+
+    def _draw(self, shape):
+        """(axis, lo, hi) of the next call."""
+        seed = None if self.seed is None else self.seed + self._calls
+        self._calls += 1
+        return augment._draw_crop(list(shape), self.crop_min, self.crop_max, self.axis, self.prob, self.bilateral,
+                                  seed)
+
+    def call(self, x):
+        if self.prob == 0:
+            return x
+        require_cuda(x)
+        if x.dtype not in (torch.float32, torch.int32):
+            raise NotImplementedError(f'RandomCrop: fp32 or int32 input, got {x.dtype}')
+        axis, lo, hi = self._draw(x.shape)
+        if x.dtype == torch.int32:
+            return _crop_window(x.contiguous(), axis, lo, hi)
+        return _CropFn.apply(x, axis, lo, hi)
 
 
 # ---------------------------------------------------------------------------------------

@@ -684,4 +684,54 @@ def subsample_axis(x, stride_min=1, stride_max=8, axes=None, prob=1, upsample=Tr
     return gather_axis(x, subsample_indices(x.shape[ax], thick, upsample), ax)
 
 
+def _item_minmax(x2d):
+    """device [items, 2] = per-row (min, max) of the contiguous fp32 [items, n] view x2d (nrt_item_minmax_f32)."""
+    items, n = x2d.shape
+    mnmx = torch.empty(items, 2, dtype=torch.float32, device=x2d.device)
+    nb = lib.nrt_item_minmax_workspace_bytes(int(items), int(n))
+    ws = _scratch(x2d.device, nb)
+    with torch.cuda.device(x2d.device):
+        check(lib.nrt_item_minmax_f32(ptr(x2d), int(items), int(n), ptr(mnmx), ptr(ws), nb, stream_ptr(x2d.device)))
+    return mnmx
+
+
+def _norm_gamma(x2d, C, mnmx, gamma_u=None, gamma=0.0):
+    """[items, n] -> div_no_nan(x - mn, mx - mn) per row (mnmx may be None: no normalisation), then
+    pow(., u * (2 gamma) + (1 - gamma)) with gamma_u [items, C] when given (nrt_norm_gamma_f32)."""
+    items, n = x2d.shape
+    out = torch.empty_like(x2d)
+    f32 = np.float32
+    with torch.cuda.device(x2d.device):
+        check(lib.nrt_norm_gamma_f32(ptr(x2d), int(items), int(n), int(C), ptr(mnmx), ptr(gamma_u),
+                                     float(f32(1 - gamma)), float(f32(1 + gamma)), ptr(out), stream_ptr(x2d.device)))
+    return out
+
+
+def minmax_norm(x, axis=None):
+    """Min-max normalize x with a safe division (utils.py:953-968): (x - min) / (max - min), 0 where max == min,
+    the extrema taken over `axis` (None: all).  Built for axis=None and any set of trailing axes; the extrema
+    stay on the device."""
+    require_cuda(x)
+    if x.requires_grad and torch.is_grad_enabled():
+        raise RuntimeError('minmax_norm has no gradient path through the extrema; pass a detached input')
+    nd = x.dim()
+    if axis is None:
+        k = 0
+    else:
+        axes = sorted({int(a) + nd if int(a) < 0 else int(a) for a in np.ravel(axis)})
+        if any(a < 0 or a >= nd for a in axes):
+            raise ValueError(f'axis {axis} out of range for a rank-{nd} tensor')
+        k = nd - len(axes)
+        if axes != list(range(k, nd)):
+            raise NotImplementedError(f'minmax_norm: only axis=None or trailing axes are built, got {axis}')
+    x32 = _as_f32(x).contiguous()
+    items = int(np.prod(x32.shape[:k], dtype=np.int64))
+    n = int(np.prod(x32.shape[k:], dtype=np.int64))
+    if x32.numel() == 0:
+        return x32.clone()
+    x2d = x32.reshape(items, n)
+    out = _norm_gamma(x2d, 1, _item_minmax(x2d)).reshape(x32.shape)
+    return out.to(x.dtype) if x.dtype.is_floating_point and x.dtype != torch.float32 else out
+
+
 from . import augment  # noqa: E402,F401  (ne.utils.augment.*, as in the reference)

@@ -462,10 +462,85 @@ def gen_noise():
             **{k: v for k, v in kw.items()})
 
 
+SYNTH_CASES = {  # name: (batch, labels drawn from, labels_to_image_new kwargs)
+    'synth_3d_defaults_b2': (2, [0, 1, 2, 4], dict(
+        labels_in=[0, 1, 2, 4], in_shape=(10, 12, 14), return_vel=True, return_def=True, return_mean=True,
+        return_bias=True)),
+    'synth_2d_dict_int_bg': (2, [0, 1, 2, 5, 7], dict(
+        labels_in={0: 0, 1: 1, 2: 1, 5: 2, 7: 3}, labels_out={1: 1, 5: 2, 7: 2}, in_shape=(20, 22), num_chan=2,
+        mean_min=[0, 0.2, 0.4, 0.6], mean_max=[0.1, 0.5, 0.6, 1.0], one_hot=False, crop_prob=1, crop_axes=1,
+        zero_background=1, noise_max=0, gamma=0, slice_prob=1, return_mean=True)),
+    'synth_3d_half_res_out': (1, [0, 1, 2, 3], dict(
+        labels_in=[0, 1, 2, 3], in_shape=(12, 12, 16), out_shape=(10, 10, 12), half_res=True, warp_max=0, bias_max=0,
+        normalize=False, gamma=0, crop_prob=1, crop_max=0.5, return_def=False, return_mean=True)),
+    'synth_2d_list_gaps_gamma': (1, [0, 3, 5, 9], dict(
+        labels_in=[0, 3, 5, 9], in_shape=(18, 16), crop_prob=1, crop_max=0.5, slice_prob=1, noise_max=0,
+        zero_background=0, warp_max=0, return_mean=True, return_bias=True)),
+    'synth_3d_noise_bg_nonorm': (1, [0, 1, 2], dict(
+        labels_in=[0, 1, 2], in_shape=(8, 10, 12), zero_background=1, normalize=False, gamma=0, blur_max=0,
+        bias_max=0, return_mean=True)),
+}
+CROP_CASES = {  # name: (input shape, dtype, RandomCrop kwargs)
+    'crop_2d_bilateral_prob': ((2, 17, 23, 1), 'float32', dict(crop_min=0.1, crop_max=0.6, axis=2, prob=0.7,
+                                                               bilateral=True)),
+    'crop_3d_int_all_axes': ((1, 9, 11, 13, 2), 'int32', dict(crop_min=0.2, crop_max=0.4)),
+    'crop_3d_axis_subset': ((2, 8, 10, 12, 1), 'float32', dict(crop_max=0.5, axis=[1, 3], prob=1)),
+}
+
+
+def gen_synth():
+    """The reference's own labels_to_image_new, RandomCrop, draw_crop_mask and minmax_norm on replayed draws, with
+    tools/vxmstub.py as voxelmorph (provenance 'contract' for the warp chain, as the st_* fixtures)."""
+    import vxmstub
+    vxmstub.install()
+    rng = np.random.default_rng(123)
+    ref = ('reference neurite/tf/models.py:920-1301 labels_to_image_new on tfshim + tools/vxmstub.py (voxelmorph '
+           'warp chain: contract), tf.random replayed from the stored draws')
+
+    class InputModel:
+        def __init__(self, x):
+            self.output, self.inputs = T(x), [T(x)]
+
+    def log():
+        return {'q%d' % i: d for i, d in enumerate(tfshim.REPLAY.log)}
+
+    for name, (B, labs, kw) in SYNTH_CASES.items():
+        x = rng.choice(np.asarray(labs), (B,) + tuple(kw['in_shape']) + (1,)).astype(np.int32)
+        tfshim.REPLAY = tfshim.Replay(rng)
+        args = dict(kw)
+        args.pop('in_shape')
+        outs = ne.models.labels_to_image_new(input_model=InputModel(x), **args)
+        outs = outs if isinstance(outs, list) else [outs]
+        q = log()
+        save(name, ref, labels=x, kwargs=np.array(repr(kw)), nout=np.array(len(outs)),
+             **{'out%d' % i: npy(o) for i, o in enumerate(outs)}, nq=np.array(len(q)), **q)
+
+    ref_c = 'reference neurite/tf/layers.py:446-519 RandomCrop, utils/augment.py:221-287 on tfshim, draws replayed'
+    for name, (shape, dt, kw) in CROP_CASES.items():
+        x = (rng.integers(-5, 6, shape) if dt == 'int32' else rng.standard_normal(shape)).astype(dt)
+        tfshim.REPLAY = tfshim.Replay(rng)
+        out = npy(ne.layers.RandomCrop(**kw)(T(x)))
+        q = log()
+        save(name, ref_c, x=x, out=out, kwargs=np.array(repr(kw)), nq=np.array(len(q)), **q)
+    xm = rng.standard_normal((3, 7, 5)).astype(F32)
+    tfshim.REPLAY = tfshim.Replay(rng)
+    m = npy(ne.utils.augment.draw_crop_mask(T(xm), crop_min=0.3, crop_max=0.3, axis=None, prob=1))
+    q = log()
+    save('crop_mask_fixed_prop', ref_c, x=xm, out=m, kwargs=np.array(repr(dict(crop_min=0.3, crop_max=0.3))),
+         nq=np.array(len(q)), **q)
+
+    ref_m = 'reference neurite/tf/utils/utils.py:953-968 minmax_norm on tfshim'
+    for name, shape, axis in (('minmax_all', (2, 9, 11, 3), None), ('minmax_trailing', (3, 8, 7, 2), (1, 2, 3))):
+        x = (2 * rng.standard_normal(shape) + 1).astype(F32)
+        save(name, ref_m, x=x, out=npy(ne.utils.minmax_norm(T(x), axis=axis)), axis=np.array(repr(axis)))
+    xc = np.full((2, 4, 5), 3.0, F32)
+    save('minmax_constant', ref_m, x=xc, out=npy(ne.utils.minmax_norm(T(xc))), axis=np.array('None'))
+
+
 if __name__ == '__main__':
     only = sys.argv[2:]
     for fn in (gen_interpn, gen_resize, gen_spatial_transformer, gen_dice, gen_lc3d, gen_lc3d_impl, gen_mi, gen_blur,
-               gen_noise):
+               gen_noise, gen_synth):
         if not only or fn.__name__[4:] in only:
             fn()
     tot = sum(os.path.getsize(os.path.join(OUT, f)) for f in os.listdir(OUT))

@@ -187,6 +187,10 @@ class Tensor:
     def __truediv__(self, o): return self._bin(o, np.true_divide)
     def __rtruediv__(self, o): return self._bin(o, np.true_divide, True)
     def __neg__(self): return Tensor(-self._a)
+    # matrix products (models.py:1117, affine chain): float64 numpy matrices with an fp32 tensor; the result is
+    # cast back to the tensor's dtype (exact for the identity affine with integer / half-integer shifts in scope)
+    def __matmul__(self, o): return Tensor(np.matmul(self._a, A(o)).astype(self._a.dtype))
+    def __rmatmul__(self, o): return Tensor(np.matmul(A(o), self._a).astype(self._a.dtype))
     def __pow__(self, o): return self._bin(o, np.power)
     def __lt__(self, o): return self._bin(o, np.less)
     def __le__(self, o): return self._bin(o, np.less_equal)
@@ -303,6 +307,16 @@ REPLAY = Replay()
 
 def _uniform(shape, minval=0, maxval=None, dtype=None, seed=None, **k):
     dt = np.float32 if dtype is None else _np_dtype(dtype)
+    if np.issubdtype(dt, np.integer):
+        # integer draws replay the integer itself: U{minval, ..., maxval - 1}
+        lo, hi = int(A(T(minval))), int(A(T(maxval)))
+        if REPLAY.queue:
+            i = REPLAY.take('int', shape)
+        else:
+            i = REPLAY.rng.integers(lo, hi, tuple(int(v) for v in np.ravel(A(T(shape))))).astype(np.float32)
+            REPLAY.log.append(i)
+        assert np.all((lo <= i) & (i < hi)), 'replayed integer draw outside [%d, %d)' % (lo, hi)
+        return Tensor(np.asarray(i).astype(dt))
     lo = np.asarray(A(T(minval)), dt)
     hi = np.asarray(A(T(1 if maxval is None else maxval)), dt)
     u = REPLAY.take('uniform', shape).astype(dt)
@@ -582,6 +596,60 @@ def _install_tf():
     losses.MeanSquaredError = MeanSquaredError
     keras.losses = losses
     tf.keras = keras
+
+    # ---- additions for labels_to_image_new / RandomCrop / draw_crop_mask / minmax_norm (eager only) ----
+    _concat = tf.concat
+    tf.concat = lambda vals, axis, **k: vals if isinstance(vals, Tensor) else _concat(vals, axis)
+    tf.gather = lambda params, indices, axis=0, **k: Tensor(np.take(A(T(params)), A(T(indices)), axis=int(A(T(axis)))))
+    tf.equal = lambda a, b: Tensor(np.equal(A(T(a)), A(T(b))))
+    tf.greater_equal = lambda a, b: Tensor(np.greater_equal(A(T(a)), A(T(b))))
+    tf.logical_and = lambda a, b: Tensor(np.logical_and(A(T(a)), A(T(b))))
+    tf.pow = lambda a, b: Tensor(np.power(A(T(a)), A(T(b))).astype(A(T(a)).dtype))
+    tfmath.less = tf.less
+    tfmath.logical_and = tf.logical_and
+    tfmath.logical_xor = lambda a, b: Tensor(np.logical_xor(A(T(a)), A(T(b))))
+    tf.reduce_min = lambda x, axis=None, keepdims=False: Tensor(np.min(A(T(x)), axis=axis, keepdims=keepdims))
+    tf.reduce_max = lambda x, axis=None, keepdims=False: Tensor(np.max(A(T(x)), axis=axis, keepdims=keepdims))
+    v1.div_no_nan = divide_no_nan
+
+    def one_hot(indices, depth, dtype=None, **k):
+        out = A(K.one_hot(indices, int(depth)))
+        return Tensor(out.astype(np.float32 if dtype is None else _np_dtype(dtype)))
+    tf.one_hot = one_hot
+
+    def roll(x, shift, axis):
+        return Tensor(np.roll(np.asarray([float(A(T(v))) for v in x]), int(A(T(shift))), axis=int(axis)))
+    tf.roll = roll
+
+    def range_(start, limit=None, delta=1, dtype=None, **k):
+        # tf.range with a float delta (provenance: contract; TF's RangeOp, restated): size ceil(|limit - start| /
+        # |delta|) and element start + i * delta, each op rounded once in the arguments' dtype
+        if limit is None:
+            start, limit = 0, start
+        if dtype is None and isinstance(delta, Tensor) and A(delta).dtype.kind == 'f':
+            dt = A(delta).dtype.type
+            s, l, d = dt(A(T(start))), dt(A(T(limit))), dt(A(T(delta)))
+            n = int(np.ceil(np.abs(dt(dt(l - s) / d))))
+            return Tensor((s + np.arange(n, dtype=dt) * d).astype(dt))
+        return Tensor(np.arange(A(T(start)), A(T(limit)), A(T(delta)),
+                                dtype=np.int32 if dtype is None else _np_dtype(dtype)))
+    tf.range = range_
+
+    class _Policy:
+        compute_dtype = 'float32'
+    mp = _InertModule('tensorflow.keras.mixed_precision')
+    mp.global_policy = lambda: _Policy()
+    keras.mixed_precision = mp
+    layers.Lambda = lambda fn, **k: (lambda x: fn(x))
+
+    class Model(_InertBase):
+        """tf.keras.Model(inputs, outputs) in eager replay: the outputs themselves; a base class otherwise."""
+
+        def __new__(cls, *a, **k):
+            if cls is Model and (len(a) >= 2 or 'outputs' in k):
+                return a[1] if len(a) >= 2 else k['outputs']
+            return object.__new__(cls)
+    keras.Model = Model
 
     mods = {
         'tensorflow': tf, 'tensorflow.math': tfmath, 'tensorflow.debugging': dbg,
