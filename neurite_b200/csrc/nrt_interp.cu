@@ -160,14 +160,9 @@ resize3d_kernel(const float* __restrict__ vol, float* __restrict__ out, ResizeGe
   __syncthreads();
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const int ox = x0 + lane, oy = y0 + wid;
-  // C = 3: a warp's row is 96 contiguous floats; the lanes exchange their 3 channels through
-  // shared memory so that the row leaves as three fully coalesced 128-byte stores instead of
-  // three 12-byte-strided ones (3x fewer L2 write sectors).  All lanes of a row take part, so
-  // lanes past the x end keep running on the zero table entry (offset 0, weights 0).
-  // (compiled out: the two warp syncs cost more than the write sectors they save)
-  constexpr bool kRowStore = false && (METHOD == NRT_LINEAR && CT == 3);
-  __shared__ float s_row[kRowStore ? 8 * 96 : 1];
-  if (oy >= w.M[1] || (!kRowStore && ox >= w.M[2])) return;
+  // (C = 3 rows exchanged through shared memory for coalesced 128-byte stores were tried: the warp syncs cost more
+  // than the write sectors they saved)
+  if (oy >= w.M[1] || ox >= w.M[2]) return;
   const AxisEntry ey = s_ax[TZ + wid], ex = s_ax[TZ + TY + lane];
   const float* volb = vol + (size_t)b * w.src_batch_stride;
   float* outb = out + ((size_t)b * w.out_vox + ((size_t)z0 * w.M[1] + oy) * w.M[2] + ox) * C;
@@ -183,7 +178,6 @@ resize3d_kernel(const float* __restrict__ vol, float* __restrict__ out, ResizeGe
     constexpr int CN = CT > 0 ? CT : 1;
     float lo[4][CN], hi[4][CN];
     int cur0 = -1, cur1 = -1;
-    const int nrow = min(32, w.M[2] - x0) * 3;           // floats of this warp's row that exist (row store)
 #pragma unroll 1
     for (int z = 0; z < TZ; ++z, outb += plane) {
       if (z0 + z >= w.out_n0) break;
@@ -235,16 +229,7 @@ resize3d_kernel(const float* __restrict__ vol, float* __restrict__ out, ResizeGe
         r = __fadd_rn(r, __fmul_rn(k7, hi[3][c]));
         res[c] = r;
       }
-      if (kRowStore) {
-        float* so = s_row + wid * 96;
-        so[lane * 3 + 0] = res[0]; so[lane * 3 + 1] = res[1]; so[lane * 3 + 2] = res[2];
-        __syncwarp();
-        float* rowp = outb - lane * 3;                        // first float of the warp's row
-#pragma unroll
-        for (int m = 0; m < 3; ++m)
-          if (lane + 32 * m < nrow) st_stream_f(rowp + lane + 32 * m, so[lane + 32 * m]);
-        __syncwarp();
-      } else if (CT == 4) {
+      if (CT == 4) {
         *reinterpret_cast<float4*>(outb) = make_float4(res[0], res[1], res[2], res[3]);     // 16-byte aligned: 4 floats per voxel
       } else if (CT == 2) {
         *reinterpret_cast<float2*>(outb) = make_float2(res[0], res[1]);

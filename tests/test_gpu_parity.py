@@ -503,10 +503,15 @@ def test_vxm_adjacent_transforms_vs_oracle(ne):
         np.testing.assert_array_equal(out, ointerp.rescale_transform(half, z))
 
 
+# the last four stage their source (S2·C % 4 == 0) but their voxel pairs cannot leave as 64 / 128-bit stores -- row
+# pitch 35, 70 and 105 floats, and an even pitch with an item stride of 90 floats -- so they take the one-voxel staged
+# kernel by default
 @pytest.mark.parametrize('shape,C,zoom', [((7, 9, 33), 1, 2), ((6, 5, 40), 2, 3), ((5, 6, 35), 3, 2.5), ((4, 7, 34), 4, 4),
                                           ((9, 8, 32), 3, [1.5, 2, 3.7]), ((3, 2, 2), 1, 2), ((10, 12, 70), 3, 1.6),
                                           ((40, 9, 21), 3, [2, 2, 3]), ((5, 33, 17), 2, 2), ((6, 7, 9), 1, [2, 2, 0.6]),
-                                          ((33, 18, 20), 4, [0.5, 1.3, 2.1])])
+                                          ((33, 18, 20), 4, [0.5, 1.3, 2.1]), ((6, 7, 20), 1, [2, 2, 1.75]),
+                                          ((5, 6, 20), 2, [2, 2, 1.75]), ((5, 6, 20), 3, [2, 2, 1.75]),
+                                          ((3, 3, 8), 1, [1, 1, 1.25])])
 def test_resize_upsampling_vs_oracle(ne, monkeypatch, shape, C, zoom):
     """up-sampling (and mixed) shapes through the TMA-staged tile kernels (voxel-pair kernel: default, even and odd
     output widths, and its global-memory path; one voxel per thread), the one-voxel z-marching kernel (global loads)
@@ -530,6 +535,31 @@ def test_resize_upsampling_vs_oracle(ne, monkeypatch, shape, C, zoom):
     np.testing.assert_array_equal(ne.layers.Resize(zoom)(dev(x)).cpu().numpy(), ref)
     monkeypatch.setenv('NRT_RESIZE_GENERIC', '1')
     np.testing.assert_array_equal(ne.layers.Resize(zoom)(dev(x)).cpu().numpy(), ref)
+
+
+@pytest.mark.parametrize('C', [1, 2, 3, 4])
+def test_resize_unaligned_output_vs_oracle(ne, C):
+    """nrt_resize_f32 into an output one float past an aligned allocation, from a TMA-able source (S2·C % 4 == 0):
+    C = 1, 3 take the one-voxel staged kernel, C = 2, 4 the run-time-C z-marching kernel.  Bit-exact incl. the sign of
+    zero, and nothing written outside the output"""
+    from neurite_b200._lib import lib, check, ptr, stream_ptr, i32_array, method_id
+    rng = np.random.default_rng(52)
+    shape, zoom = (5, 6, 20), [2, 2, 1.75]
+    x = rng.standard_normal((2,) + shape + (C,)).astype(F32)
+    x[0, 0, 0, :2] = 0.0
+    x[1, -1, -1, -3:] = -0.0
+    ref = ointerp.resize_layer(x, zoom)
+    new_shape = ref.shape[1:4]
+    buf = torch.full((ref.size + 2,), float('nan'), device='cuda')
+    out = buf[1:1 + ref.size]
+    assert out.data_ptr() % 16 == 4
+    xd = dev(x)
+    check(lib.nrt_resize_f32(ptr(xd), ptr(out), 2, i32_array(shape), i32_array(new_shape), 3, C,
+                             method_id('linear'), 0, new_shape[0], stream_ptr()))
+    got = out.cpu().numpy().reshape(ref.shape)
+    np.testing.assert_array_equal(got, ref)
+    np.testing.assert_array_equal(np.signbit(got), np.signbit(ref))
+    assert torch.isnan(buf[0]) and torch.isnan(buf[-1])
 
 
 def test_interpn_on_the_volume_grid_uses_tiles_and_stays_exact(ne, monkeypatch):
