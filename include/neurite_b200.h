@@ -341,6 +341,14 @@ NRT_API int nrt_crop_window_f32(const float* x, int64_t outer, int64_t L, int64_
                           float* out, void* stream);
 NRT_API int nrt_crop_window_i32(const int32_t* x, int64_t outer, int64_t L, int64_t inner, int64_t lo, int64_t hi,
                           int32_t* out, void* stream);
+/* The generator's label warp (models.py:1130-1160) in one pass: labels [B, *in_shape, 1] fp32, mats [B, N, N+1] fp32
+ * (one affine per item), def [B, *out_shape, N] fp32 or null -> out [B, *out_shape, 1], N = 2 or 3.  With the dense
+ * shift s_i(c) = ((M_i0 c_0 + M_i1 c_1) + M_i2 c_2) + M_iN - c_i at integer out-grid points c, t = s(x) without def
+ * and t = def(x) + interpn_linear(s, x + def(x)) with it; out = the nearest sample of the labels at x + t, 0 outside
+ * the in grid.  Every op is rounded once: bit for bit AffineToDenseShift, ComposeTransform and the nearest
+ * SpatialTransformer with fill 0. */
+NRT_API int nrt_warp_labels_affine_f32(const float* labels, const float* mats, const float* def, float* out, int B,
+                          int N, const int32_t* in_shape, const int32_t* out_shape, void* stream);
 
 #ifdef __cplusplus
 }

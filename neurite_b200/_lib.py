@@ -101,6 +101,8 @@ SIGNATURES = {
                                           c_vp, c_vp]),
     'nrt_crop_window_f32': (ctypes.c_int, [c_vp, c_i64, c_i64, c_i64, c_i64, c_i64, c_vp, c_vp]),
     'nrt_crop_window_i32': (ctypes.c_int, [c_vp, c_i64, c_i64, c_i64, c_i64, c_i64, c_vp, c_vp]),
+    'nrt_warp_labels_affine_f32': (ctypes.c_int, [c_vp, c_vp, c_vp, c_vp, ctypes.c_int, ctypes.c_int, P_I32, P_I32,
+                                                   c_vp]),
 }
 
 

@@ -6,29 +6,32 @@ neurite_b200.models -- the SynthMorph / SynthSeg image generator of neurite
     image, label_map = gen(labels)            # labels [B, *in_shape, 1], integer or float
 
 Stages and where they run:
-    velocity PerlinNoise -> VecInt(5) -> RescaleTransform(2) -> ComposeTransform -> nearest SpatialTransformer
-                                              the existing layers
+    affine parameters, flip, swap, the composed [B, N, N+1] matrix     host (numpy), one copy to the device
+    velocity PerlinNoise -> VecInt(5) -> RescaleTransform(2)          the existing layers
+    dense affine shift, composition with the deformation, nearest label warp
+                                              nrt_warp_labels_affine_f32 (one pass)
     crop, generation LUT, per-label means, exp(bias), max |image|     nrt_labels_to_image_f32 (one pass)
     GaussianNoise (+ background clearing)     nrt_philox_normal_f32 / nrt_philox_normal_background_f32
     random GaussianBlur, Subsample            utils.separable_conv, utils.gather_axis
     per-item min / max, normalisation, gamma  nrt_item_minmax_f32, nrt_norm_gamma_f32
     crop, output LUT, one-hot / int map       nrt_label_map_f32 / nrt_label_map_i32
 
-Randomness.  Every component (warp, crop, mean, bias, noise, background, blur, slice, gamma) takes its seed from
-`seeds` and draws with `seed + number of earlier calls`, like the layers; `seed=None` seeds from the operating
-system.  An iterable of names seeds each with `hash(name)`, as the reference does; Python salts the hash of a
-string per process (PYTHONHASHSEED), so such seeds repeat only within one process.  Small draws are made on the
-host with numpy (crop, blur SDs, subsample); the tables (per-label mean U [B, C, N], background U [B], gamma
-U [B, C]) are drawn on the device by the Philox stream of nrt_noise.cu, and TF's fp32 `u * (max - min) + min` is
-applied in the kernel that reads them.  A call makes no device-to-host copy and leaves torch's RNG untouched.
+Randomness.  Every component (shift, rot, scale, shear, flip, swap, warp, crop, mean, bias, noise, background,
+blur, slice, gamma) takes its seed from `seeds` and draws with `seed + number of earlier calls`, like the layers;
+`seed=None` seeds from the operating system.  An iterable of names seeds each with `hash(name)`, as the reference
+does; Python salts the hash of a string per process (PYTHONHASHSEED), so such seeds repeat only within one
+process.  Small draws are made on the host with numpy (affine, flip, swap, crop, blur SDs, subsample); the tables
+(per-label mean U [B, C, N], background U [B], gamma U [B, C]) are drawn on the device by the Philox stream of
+nrt_noise.cu, and TF's fp32 `u * (max - min) + min` is applied in the kernel that reads them.  A call makes no
+device-to-host copy and leaves torch's RNG untouched.
 
 A call is `_synthesize(labels, _draw(labels))`: `_draw` makes every random quantity (the plan), `_synthesize` is
 deterministic given it.
 
-Scope: the affine draw of the reference comes from voxelmorph (DrawAffineParams, draw_flip_matrix,
-draw_swap_matrix) and is not built: non-zero aff_*, axes_flip, axes_swap and input_model raise
-NotImplementedError.  The origin / center / scale matrices at identity affine are applied, so out_shape and
-half_res work.
+The affine.  The reference takes DrawAffineParams, ParamsToAffineMatrix, draw_flip_matrix and draw_swap_matrix
+from voxelmorph; they are restated here as a contract (DESIGN.md §2): affine_params, affine_matrix, flip_matrix,
+swap_matrix and compose_affine below, used when the builder is given vxm_affine=True.  Bounds must be scalars;
+input_model raises NotImplementedError.
 """
 import numpy as np
 import torch
@@ -38,10 +41,106 @@ from ._lib import lib, check, ptr, stream_ptr, i32_array, require_cuda
 
 _MAX_SEED = np.iinfo(int).max
 _COMPONENTS = ('warp', 'crop', 'mean', 'bias', 'noise', 'background', 'blur', 'slice', 'gamma')
+_AFFINE = ('shift', 'rot', 'scale', 'shear')
+F32 = np.float32
 
 
 def _key(seed):
     return int(np.random.default_rng(seed).integers(_MAX_SEED))
+
+
+# ---- the affine draw (voxelmorph's DrawAffineParams, ParamsToAffineMatrix, draw_flip_matrix, draw_swap_matrix) ----
+def affine_sizes(ndims):
+    """Parameters per item and kind: shift N, rotation 3 (1 in 2-D), scale N, shear 3 (1 in 2-D)."""
+    r = 3 if ndims == 3 else 1
+    return {'shift': ndims, 'rot': r, 'scale': ndims, 'shear': r}
+
+
+def affine_params(batch, ndims, bounds, normal, seeds):
+    """[batch, 12] (3-D) or [batch, 6] (2-D) fp32 parameters, in the order shift, rotation (degrees), scale, shear.
+    Each kind draws from numpy's generator seeded with seeds[kind]: uniform on [-bound, bound] as TF's fp32
+    u * (2 bound) - bound, or with normal[kind] z * bound, the scale's z redrawn where |z| > 2 (truncated at 2 SD).
+    A bound of 0 draws nothing and gives zeros."""
+    out = []
+    for kind, n in affine_sizes(ndims).items():
+        b, shape = float(bounds[kind]), (batch, n)
+        if b == 0:
+            out.append(np.zeros(shape, F32))
+            continue
+        rng = np.random.default_rng(seeds.get(kind))
+        if not normal[kind]:
+            out.append((rng.random(shape, dtype=F32) * F32(2 * b) + F32(-b)).astype(F32))
+            continue
+        z = rng.standard_normal(shape, dtype=F32)
+        while kind == 'scale' and np.any(np.abs(z) > 2):
+            bad = np.abs(z) > 2
+            z[bad] = rng.standard_normal(int(bad.sum()), dtype=F32)
+        out.append((z * F32(b)).astype(F32))
+    return np.concatenate(out, 1)
+
+
+def affine_matrix(params, ndims):
+    """ParamsToAffineMatrix(deg=True, shift_scale=True, last_row=True): [B, N+1, N+1] fp32 with A = R (Z S),
+    Z = diag(1 + scale), S the upper unit-triangular shear, R = Rx (Ry Rz) in 3-D, and the shift as the last
+    column; evaluated in fp64, rounded once."""
+    p = np.asarray(params, np.float64)
+    n = affine_sizes(ndims)
+    shift, rot = p[:, :ndims], np.deg2rad(p[:, ndims:ndims + n['rot']])
+    scale, shear = p[:, ndims + n['rot']:2 * ndims + n['rot']], p[:, 2 * ndims + n['rot']:]
+    out = np.zeros((p.shape[0], ndims + 1, ndims + 1))
+    for b in range(p.shape[0]):
+        c, s = np.cos(rot[b]), np.sin(rot[b])
+        if ndims == 3:
+            rx = np.array([[1, 0, 0], [0, c[0], -s[0]], [0, s[0], c[0]]])
+            ry = np.array([[c[1], 0, s[1]], [0, 1, 0], [-s[1], 0, c[1]]])
+            rz = np.array([[c[2], -s[2], 0], [s[2], c[2], 0], [0, 0, 1]])
+            r = rx @ (ry @ rz)
+            sh = np.array([[1, shear[b, 0], shear[b, 1]], [0, 1, shear[b, 2]], [0, 0, 1]])
+        else:
+            r = np.array([[c[0], -s[0]], [s[0], c[0]]])
+            sh = np.array([[1, shear[b, 0]], [0, 1]])
+        out[b, :ndims, :ndims] = r @ (np.diag(1 + scale[b]) @ sh)
+        out[b, :ndims, ndims] = shift[b]
+        out[b, ndims, ndims] = 1
+    return out.astype(F32)
+
+
+def draw_flip(seed, ndims):
+    """The flipped axes [ndims] bool: each with probability 1/2 (U[0, 1) > 0.5)."""
+    return np.random.default_rng(seed).random(ndims, dtype=F32) > 0.5
+
+
+def draw_swap(seed, ndims):
+    """A uniformly random permutation of the axes."""
+    return np.random.default_rng(seed).permutation(ndims)
+
+
+def flip_matrix(flip, out_shape):
+    """draw_flip_matrix(out_shape, shift_center=False) given the flipped axes: x -> (out_shape - 1) - x there."""
+    n = len(out_shape)
+    m = np.eye(n + 1)
+    for a in np.flatnonzero(flip):
+        m[a, a], m[a, n] = -1, out_shape[a] - 1
+    return m
+
+
+def swap_matrix(perm):
+    """draw_swap_matrix given the permutation: P[i, perm[i]] = 1."""
+    n = len(perm)
+    m = np.eye(n + 1)
+    m[:n, :n] = np.eye(n)[list(perm)]
+    return m
+
+
+def compose_affine(aff, pre, post, flip=None, swap=None):
+    """The matrix the warp applies (models.py:1117-1131): (((pre @ aff) @ post) @ flip) @ swap in fp64, top N rows
+    as fp32 [B, N, N+1].  pre = inv(origin), post = origin @ center @ scale."""
+    m = pre @ np.asarray(aff, np.float64) @ post
+    for f in (flip, swap):
+        if f is not None:
+            m = m @ f
+    n = m.shape[-1] - 1
+    return np.ascontiguousarray(m[:, :n, :]).astype(F32)
 
 
 def _uniform01(key, shape, device):
@@ -83,7 +182,7 @@ class LabelsToImage(torch.nn.Module):
         super().__init__()
         self.cfg = cfg
         self._calls = 0
-        self._shift_cache = {}
+        self._ident_dev = {}
         c = cfg
         N = c['num_dim']
         self.vel_layer = None
@@ -123,7 +222,24 @@ class LabelsToImage(torch.nn.Module):
         dev = labels.device
         B, C, Nl = labels.shape[0], c['num_chan'], len(c['labels_gen'])
         out_shape = [int(s) for s in c['out_shape']]
+        N = c['num_dim']
         plan = {}
+        if any(v != 0 for v in c['aff_bounds'].values()) or c['axes_flip'] or c['axes_swap']:
+            params = affine_params(B, N, c['aff_bounds'], c['aff_normal'], {t: self._seed(t) for t in _AFFINE})
+            aff = affine_matrix(params, N)
+            flip = swap = None
+            if c['axes_flip']:       # one matrix per call, shared by the batch
+                flip = flip_matrix(draw_flip(self._seed('flip'), N), out_shape)
+            if c['axes_swap']:
+                swap = swap_matrix(draw_swap(self._seed('swap'), N))
+            trans = compose_affine(aff, c['aff_pre'], c['aff_post'], flip, swap)
+            # both matrices in one pinned buffer and one asynchronous copy: the host does not wait for the stream
+            host = torch.from_numpy(np.concatenate([aff.ravel(), trans.ravel()])).pin_memory()
+            mats = host.to(dev, non_blocking=True)
+            plan['aff'] = mats[:aff.size].view(B, N + 1, N + 1)
+            plan['trans'] = mats[aff.size:].view(B, N, N + 1)
+        else:                        # nothing random: the identity's matrices, cached on the device
+            plan['aff'], plan['trans'] = self._identity(dev, B)
         plan['vel'] = self.vel_layer(labels) if self.vel_layer is not None else None
         plan['crop'] = None
         if c['crop_prob'] != 0:
@@ -161,14 +277,16 @@ class LabelsToImage(torch.nn.Module):
         return plan
 
     # ---- the deterministic rest ----
-    def _affine_shift(self, device):
-        """Dense shift of the identity affine with the origin / center / scale matrices, [1, *out_shape, N]."""
-        key = (device.type, device.index)
-        if key not in self._shift_cache:
-            mat = torch.as_tensor(self.cfg['trans'][None, :self.cfg['num_dim'], :], dtype=torch.float32, device=device)
-            st = layers.SpatialTransformer(shift_center=False)
-            self._shift_cache[key] = st._affine_to_dense(mat, tuple(int(s) for s in self.cfg['out_shape']))
-        return self._shift_cache[key]
+    def _identity(self, device, batch):
+        """The identity affine [B, N+1, N+1] and its warp matrix (origin, center and scale only) [B, N, N+1], on
+        the device."""
+        key = (device.type, device.index, batch)
+        if key not in self._ident_dev:
+            c = self.cfg
+            eye = np.repeat(np.eye(c['num_dim'] + 1, dtype=F32)[None], batch, 0)
+            self._ident_dev[key] = (torch.as_tensor(eye, device=device),
+                                    torch.as_tensor(compose_affine(eye, c['aff_pre'], c['aff_post']), device=device))
+        return self._ident_dev[key]
 
     def _luts(self, device):
         key = (device.type, device.index)
@@ -181,22 +299,29 @@ class LabelsToImage(torch.nn.Module):
         return self._lut_dev[key]
 
     def warp_labels(self, labels, plan):
-        """labels [B, *in_shape, 1] -> the nearest-warped fp32 label map [B, *out_shape, 1] (and the shift)."""
+        """labels [B, *in_shape, 1] -> (the nearest-warped fp32 label map [B, *out_shape, 1], the deformation or
+        None).  The affine is plan['trans'] [B, N, N+1]; a plan without it warps with the identity affine."""
         c = self.cfg
-        x = labels if labels.dtype == torch.float32 else labels.to(torch.float32)
-        B = x.shape[0]
-        trans = self._affine_shift(x.device).expand(B, *self._affine_shift(x.device).shape[1:])
-        def_field = None
+        x = (labels if labels.dtype == torch.float32 else labels.to(torch.float32)).contiguous()
+        B, N = x.shape[0], c['num_dim']
+        mats = plan.get('trans')
+        mats = self._identity(x.device, B)[1] if mats is None else mats.contiguous()
+        def_field = d = None
         if plan['vel'] is not None:
             vel = plan['vel']
             if c['warp_zero_mean']:
-                vel = vel - vel.mean(dim=tuple(range(1, c['num_dim'] + 1)), keepdim=True)
+                vel = vel - vel.mean(dim=tuple(range(1, N + 1)), keepdim=True)
             def_field = layers.VecInt(int_steps=5)(vel)
             if not c['half_res']:
                 def_field = layers.RescaleTransform(zoom_factor=2)(def_field)
-            trans = layers.ComposeTransform()([trans, def_field])
-        warped = layers.SpatialTransformer(interp_method='nearest', fill_value=0)([x, trans.contiguous()])
-        return warped.contiguous(), def_field
+            d = def_field.contiguous()
+        out_shape = [int(s) for s in c['out_shape']]
+        warped = torch.empty(B, *out_shape, 1, dtype=torch.float32, device=x.device)
+        with torch.cuda.device(x.device):
+            check(lib.nrt_warp_labels_affine_f32(ptr(x), ptr(mats), ptr(d), ptr(warped), B, N,
+                                                 i32_array(x.shape[1:-1]), i32_array(out_shape),
+                                                 stream_ptr(x.device)))
+        return warped, def_field
 
     def _crop_args(self, plan):
         out_shape = [int(s) for s in self.cfg['out_shape']]
@@ -297,7 +422,10 @@ class LabelsToImage(torch.nn.Module):
         if c['return_def']:
             outputs.append(def_field)
         if c['return_aff']:
-            outputs.append(torch.eye(c['num_dim'] + 1, dtype=torch.float32, device=dev).expand(B, -1, -1).clone())
+            aff = plan.get('aff')
+            if aff is None:
+                aff = torch.eye(c['num_dim'] + 1, dtype=torch.float32, device=dev).expand(B, -1, -1)
+            outputs.append(aff.clone())
         if c['return_mean']:
             outputs.append(mean)
         if c['return_bias']:
@@ -363,11 +491,22 @@ def labels_to_image_new(
     return_mean=False,
     return_bias=False,
     id=0,
+    vxm_affine=False,
 ):
     """Build the module that augments label maps and synthesizes images from them (models.py:920-1301).  The
-    arguments, defaults and outputs are the reference's; see the module docstring for the scope and the
-    randomness.  Calling the module on a [B, *in_shape, 1] label map returns the outputs in the reference's
-    order (the tensor itself when there is one)."""
+    arguments, defaults and outputs are the reference's; see the module docstring for the randomness.  Calling
+    the module on a [B, *in_shape, 1] label map returns the outputs in the reference's order (the tensor itself
+    when there is one).
+
+    Affine augmentation (vxm_affine=True).  The reference draws the affine with voxelmorph, which is not part of
+    it; this package restates those pieces (DrawAffineParams, ParamsToAffineMatrix, draw_flip_matrix,
+    draw_swap_matrix) as a contract, and vxm_affine=True says the caller wants that restatement.  Without it,
+    non-zero aff_*, axes_flip and axes_swap raise NotImplementedError naming the argument, as before.  With it,
+    each item draws its own shift (voxels), rotation (degrees), scale (added to 1) and shear, uniform on
+    [-aff_*, aff_*], or normal with aff_* as the SD when aff_normal_* is set (the scale truncated at 2 SD).
+    axes_flip flips each axis with probability 1/2 and axes_swap permutes the axes (isotropic out_shape only);
+    both draw one matrix per call for the whole batch.  return_aff returns the drawn [B, N+1, N+1] matrix.
+    The bounds must be scalars; input_model raises NotImplementedError."""
     if isinstance(seeds, str):
         seeds = [seeds]
     if isinstance(seeds, dict):
@@ -383,28 +522,33 @@ def labels_to_image_new(
     out_shape = np.array(out_shape) // (2 if half_res else 1)
     num_dim = len(in_shape)
 
-    for name, v in (('aff_shift', aff_shift), ('aff_rotate', aff_rotate), ('aff_scale', aff_scale),
-                    ('aff_shear', aff_shear)):
-        if np.any(np.asarray(v) != 0):
-            raise NotImplementedError(f'labels_to_image_new: {name} != 0 needs the voxelmorph affine draw, '
-                                      f'which is not built')
-    for t in ('shift', 'rot', 'scale', 'shear'):
-        seeds.pop(t, None)
+    aff_bounds = {'shift': aff_shift, 'rot': aff_rotate, 'scale': aff_scale, 'shear': aff_shear}
+    aff_normal = {'shift': aff_normal_shift, 'rot': aff_normal_rotate, 'scale': aff_normal_scale,
+                  'shear': aff_normal_shear}
+    for name, v in zip(('aff_shift', 'aff_rotate', 'aff_scale', 'aff_shear'), aff_bounds.values()):
+        if np.ndim(v) != 0:
+            raise NotImplementedError(f'labels_to_image_new: {name} must be a scalar bound')
+        if v != 0 and not vxm_affine:
+            raise NotImplementedError(f'labels_to_image_new: {name} != 0 needs the restated voxelmorph affine '
+                                      f'draw; pass vxm_affine=True')
+    used = {t: seeds.pop(t, None) for t in _AFFINE}
     origin = np.eye(num_dim + 1)
     origin[:num_dim, -1] = -0.5 * (in_shape - 1)
     center = np.eye(num_dim + 1)
     center[:num_dim, -1] = np.round(0.5 * (in_shape - (2 if half_res else 1) * out_shape))
     scale = np.diag((*[2 if half_res else 1] * num_dim, 1))
-    trans = np.linalg.inv(origin) @ np.eye(num_dim + 1) @ origin @ center @ scale
     if axes_flip:
-        raise NotImplementedError('labels_to_image_new: axes_flip needs voxelmorph.utils.draw_flip_matrix, '
-                                  'which is not built')
+        if not vxm_affine:
+            raise NotImplementedError('labels_to_image_new: axes_flip needs the restated voxelmorph '
+                                      'draw_flip_matrix; pass vxm_affine=True')
+        used['flip'] = seeds.pop('flip', None)
     if axes_swap:
         assert all(x == out_shape[0] for x in out_shape), 'non-isotropic output shape'
-        raise NotImplementedError('labels_to_image_new: axes_swap needs voxelmorph.utils.draw_swap_matrix, '
-                                  'which is not built')
+        if not vxm_affine:
+            raise NotImplementedError('labels_to_image_new: axes_swap needs the restated voxelmorph '
+                                      'draw_swap_matrix; pass vxm_affine=True')
+        used['swap'] = seeds.pop('swap', None)
 
-    used = {}
     for name in _COMPONENTS:
         active = {'warp': warp_max > 0, 'bias': bias_max > 0, 'background': zero_background > 0,
                   'gamma': gamma > 0}.get(name, True)
@@ -433,8 +577,10 @@ def labels_to_image_new(
         raise NameError("labels_to_image_new: return_bias needs bias_max > 0 (no 'bias_field')")
     assert not seeds, f'unknown seeds {seeds}'
 
-    cfg = dict(num_dim=num_dim, in_shape=in_shape, out_shape=out_shape, half_res=half_res, trans=trans,
-               num_chan=int(num_chan), warp_min=warp_min, warp_max=warp_max, warp_blur_min=warp_blur_min,
+    cfg = dict(num_dim=num_dim, in_shape=in_shape, out_shape=out_shape, half_res=half_res,
+               aff_bounds=aff_bounds, aff_normal=aff_normal, axes_flip=bool(axes_flip), axes_swap=bool(axes_swap),
+               aff_pre=np.linalg.inv(origin), aff_post=origin @ center @ scale, num_chan=int(num_chan),
+               warp_min=warp_min, warp_max=warp_max, warp_blur_min=warp_blur_min,
                warp_blur_max=warp_blur_max, warp_zero_mean=warp_zero_mean, crop_min=crop_min, crop_max=crop_max,
                crop_prob=crop_prob, crop_axes=crop_axes, mean_min=mean_min, mean_max=mean_max, noise_min=noise_min,
                noise_max=noise_max, zero_background=zero_background, blur_min=blur_min, blur_max=blur_max,

@@ -537,10 +537,68 @@ def gen_synth():
     save('minmax_constant', ref_m, x=xc, out=npy(ne.utils.minmax_norm(T(xc))), axis=np.array('None'))
 
 
+_ALL3 = dict(aff_shift=3, aff_rotate=20, aff_scale=0.2, aff_shear=0.1)
+AFFSYNTH_CASES = {  # name: (batch, labels drawn from, labels_to_image_new kwargs)
+    'affsynth_3d_uniform_all': (2, [0, 1, 2, 4], dict(
+        labels_in=[0, 1, 2, 4], in_shape=(10, 12, 14), return_aff=True, return_def=True, **_ALL3)),
+    'affsynth_3d_normal_all': (2, [0, 1, 2, 3], dict(
+        labels_in=[0, 1, 2, 3], in_shape=(10, 12, 14), aff_shift=2, aff_rotate=15, aff_scale=0.3, aff_shear=0.1,
+        aff_normal_shift=True, aff_normal_rotate=True, aff_normal_scale=True, aff_normal_shear=True, bias_max=0,
+        return_aff=True)),
+    'affsynth_2d_shift': (2, [0, 1, 2], dict(labels_in=[0, 1, 2], in_shape=(20, 22), aff_shift=4, return_aff=True)),
+    'affsynth_2d_rotate_normal': (2, [0, 1, 2], dict(
+        labels_in=[0, 1, 2], in_shape=(20, 22), aff_rotate=30, aff_normal_rotate=True, return_aff=True)),
+    'affsynth_2d_scale_normal': (2, [0, 1, 2], dict(
+        labels_in=[0, 1, 2], in_shape=(18, 16), aff_scale=0.25, aff_normal_scale=True, return_aff=True)),
+    'affsynth_3d_shear': (2, [0, 1, 2], dict(labels_in=[0, 1, 2], in_shape=(10, 12, 14), aff_shear=0.2,
+                                             return_aff=True)),
+    'affsynth_3d_flip': (2, [0, 1, 2, 3], dict(labels_in=[0, 1, 2, 3], in_shape=(10, 12, 14), aff_rotate=10,
+                                               axes_flip=True, return_aff=True)),
+    'affsynth_3d_swap_iso': (2, [0, 1, 2, 3], dict(labels_in=[0, 1, 2, 3], in_shape=(10, 10, 10), aff_shift=2,
+                                                   axes_swap=True, axes_flip=True, return_aff=True)),
+    'affsynth_3d_half_res_out': (2, [0, 1, 2, 3], dict(
+        labels_in=[0, 1, 2, 3], in_shape=(12, 12, 16), out_shape=(10, 10, 12), half_res=True, aff_rotate=15,
+        aff_scale=0.1, bias_max=0, return_aff=True)),
+    'affsynth_2d_out_smaller': (2, [0, 1, 2, 5], dict(
+        labels_in=[0, 1, 2, 5], in_shape=(20, 24), out_shape=(16, 18), aff_shift=2, aff_rotate=25, aff_scale=0.15,
+        aff_shear=0.1, one_hot=False, return_aff=True)),
+    'affsynth_3d_nowarp': (2, [0, 1, 2, 3], dict(labels_in=[0, 1, 2, 3], in_shape=(10, 12, 14), warp_max=0,
+                                                 return_aff=True, **_ALL3)),
+}
+
+
+def gen_affsynth():
+    """The reference's own labels_to_image_new with random affine, flip and swap augmentation, on replayed draws,
+    with tools/vxmstub.py as voxelmorph (provenance 'contract').  Each fixture also stores the [B, N, N+1] matrix
+    the reference hands to AffineToDenseShift ('trans')."""
+    import vxmstub
+    vxmstub.install()
+    rng = np.random.default_rng(321)
+    ref = ('reference neurite/tf/models.py:920-1301 labels_to_image_new on tfshim + tools/vxmstub.py (voxelmorph '
+           'affine draw, matrices and warp chain: contract), tf.random replayed from the stored draws')
+
+    class InputModel:
+        def __init__(self, x):
+            self.output, self.inputs = T(x), [T(x)]
+
+    for name, (B, labs, kw) in AFFSYNTH_CASES.items():
+        x = rng.choice(np.asarray(labs), (B,) + tuple(kw['in_shape']) + (1,)).astype(np.int32)
+        tfshim.REPLAY = tfshim.Replay(rng)
+        vxmstub.LAST_TRANS.clear()
+        args = dict(kw)
+        args.pop('in_shape')
+        outs = ne.models.labels_to_image_new(input_model=InputModel(x), **args)
+        outs = outs if isinstance(outs, list) else [outs]
+        q = {'q%d' % i: d for i, d in enumerate(tfshim.REPLAY.log)}
+        assert len(vxmstub.LAST_TRANS) == 1
+        save(name, ref, labels=x, kwargs=np.array(repr(kw)), nout=np.array(len(outs)), trans=vxmstub.LAST_TRANS[0],
+             **{'out%d' % i: npy(o) for i, o in enumerate(outs)}, nq=np.array(len(q)), **q)
+
+
 if __name__ == '__main__':
     only = sys.argv[2:]
     for fn in (gen_interpn, gen_resize, gen_spatial_transformer, gen_dice, gen_lc3d, gen_lc3d_impl, gen_mi, gen_blur,
-               gen_noise, gen_synth):
+               gen_noise, gen_synth, gen_affsynth):
         if not only or fn.__name__[4:] in only:
             fn()
     tot = sum(os.path.getsize(os.path.join(OUT, f)) for f in os.listdir(OUT))

@@ -4,20 +4,24 @@ tools/vxmstub.py -- a test-only `voxelmorph` module for running the reference's 
 
 voxelmorph is not part of the reference; its layers are provenance 'contract' here, as the st_* fixtures are:
     VecInt / RescaleTransform / ComposeTransform / SpatialTransformer   the oracle's restatements (oracle/interp.py)
-    AffineToDenseShift(shape, shift_center=False)                      M[:N] @ [x, 1] - x on the output grid, fp32
-    DrawAffineParams                                                    zeros, no draw: the only case in scope
-    ParamsToAffineMatrix                                                identity [B, N+1, N+1] for zero parameters
+    AffineToDenseShift(shape, shift_center=False)                      oracle/affine.py dense_shift (fixed op order);
+                                                                        the matrix it receives is kept in LAST_TRANS
+    DrawAffineParams                                                    [B, n] draws per kind from the replay queue,
+                                                                        none for a zero bound (oracle/affine.py)
+    ParamsToAffineMatrix                                                oracle/affine.py affine_matrix
+    utils.draw_flip_matrix / draw_swap_matrix                           one U[0, 1) draw [N] each (oracle/affine.py)
 """
 import sys
 import types
 
 import numpy as np
 
-from oracle import interp as ointerp
+from oracle import affine as oaff, interp as ointerp
 import tfshim
 from tfshim import Tensor, A, T
 
 F32 = np.float32
+LAST_TRANS = []
 
 
 class _L:
@@ -26,17 +30,30 @@ class _L:
 
 
 class DrawAffineParams(_L):
+    """shift, rot, scale, shear: uniform on [-b, b], or normal with SD b (the scale truncated at 2 SD by redrawing
+    the whole [B, n] array and keeping the new values where |z| > 2)."""
     def __call__(self, x):
-        n = self.k['ndims']
-        return Tensor(np.zeros((A(T(x)).shape[0], 3 * n if n == 2 else 4 * n), F32))
+        n, B = self.k['ndims'], A(T(x)).shape[0]
+        out = []
+        for kind, size in oaff.sizes(n).items():
+            b = self.k.get(kind) or 0
+            if b == 0:
+                out.append(np.zeros((B, size), F32))
+                continue
+            if not self.k.get('normal_' + kind, False):
+                out.append(A(tfshim._uniform((B, size), minval=-b, maxval=b)))
+                continue
+            z = A(tfshim._normal((B, size)))
+            while kind == 'scale' and np.any(np.abs(z) > 2):
+                z = np.where(np.abs(z) > 2, A(tfshim._normal((B, size))), z)
+            out.append((z * F32(b) + F32(0)).astype(F32))
+        return Tensor(np.concatenate(out, 1))
 
 
 class ParamsToAffineMatrix(_L):
     def __call__(self, p):
-        p = A(T(p))
-        assert not np.any(p), 'only zero affine parameters are in scope'
-        n = self.k['ndims']
-        return Tensor(np.broadcast_to(np.eye(n + 1, dtype=F32), (p.shape[0], n + 1, n + 1)).copy())
+        assert self.k.get('deg') and self.k.get('shift_scale') and self.k.get('last_row')
+        return Tensor(oaff.affine_matrix(A(T(p)), self.k['ndims']))
 
 
 class AffineToDenseShift(_L):
@@ -44,11 +61,19 @@ class AffineToDenseShift(_L):
         shape = [int(s) for s in self.a[0]]
         assert self.k.get('shift_center') is False
         mat = np.asarray(A(T(mat)), F32)
-        grid = np.stack(np.meshgrid(*[np.arange(s, dtype=F32) for s in shape], indexing='ij'), -1)
-        n = len(shape)
-        loc = np.einsum('bij,...j->b...i', mat[:, :n, :n], grid).astype(F32) + mat[:, None, :n, n].reshape(
-            (mat.shape[0],) + (1,) * n + (n,))
-        return Tensor((loc - grid).astype(F32))
+        LAST_TRANS.append(mat.copy())
+        return Tensor(np.stack([oaff.dense_shift(m, shape) for m in mat], 0))
+
+
+def draw_flip_matrix(grid_shape, shift_center=True, dtype=None, seed=None):
+    assert shift_center is False
+    u = A(tfshim._uniform((len(grid_shape),)))
+    return Tensor(oaff.flip_matrix(u, [int(s) for s in grid_shape]).astype(F32))
+
+
+def draw_swap_matrix(ndims, dtype=None, seed=None):
+    u = A(tfshim._uniform((ndims,)))
+    return Tensor(oaff.swap_matrix(u).astype(F32))
 
 
 class VecInt(_L):
@@ -80,9 +105,12 @@ def install():
     for c in (DrawAffineParams, ParamsToAffineMatrix, AffineToDenseShift, VecInt, RescaleTransform,
               ComposeTransform, SpatialTransformer):
         setattr(lay, c.__name__, c)
-    vxm.layers = lay
+    utl = types.ModuleType('voxelmorph.utils')
+    utl.draw_flip_matrix, utl.draw_swap_matrix = draw_flip_matrix, draw_swap_matrix
+    vxm.layers, vxm.utils = lay, utl
     sys.modules['voxelmorph'] = vxm
     sys.modules['voxelmorph.layers'] = lay
+    sys.modules['voxelmorph.utils'] = utl
     return vxm
 
 
