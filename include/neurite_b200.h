@@ -27,7 +27,7 @@
 extern "C" {
 #endif
 
-#define NRT_ABI_VERSION 1
+#define NRT_ABI_VERSION 2
 
 #if defined(__GNUC__)
 #define NRT_API __attribute__((visibility("default")))
@@ -46,6 +46,7 @@ typedef enum {
 
 enum { NRT_LINEAR = 0, NRT_NEAREST = 1 };
 enum { NRT_ACT_LINEAR = 0, NRT_ACT_RELU = 1, NRT_ACT_SIGMOID = 2, NRT_ACT_TANH = 3 };
+enum { NRT_STAT_SD = 0, NRT_STAT_MAX = 1, NRT_STAT_ABSMAX = 2, NRT_STAT_MINMAX = 3 };
 
 NRT_API int nrt_version(void);
 NRT_API const char* nrt_last_error_string(void);
@@ -254,10 +255,8 @@ NRT_API int nrt_mi_bwd_f32(const float* x, int64_t x_batch_stride, int64_t x_vox
                    float* dcenters, void* workspace, int64_t workspace_bytes, void* stream);
 NRT_API int nrt_mi_minmax_bwd_f32(const float* x, int64_t n, const float* minmax, const float* dcenters, int nb,
                           float* grad_x, void* stream);
-/* out2 = {min(x), max(x)} over n elements (K.min / K.max, utils.py:1151-1152). */
-NRT_API int64_t nrt_minmax_workspace_bytes(void);
-NRT_API int nrt_minmax_f32(const float* x, int64_t n, float* out2, void* workspace, int64_t workspace_bytes, void* stream);
-/* centers = tf.linspace(minmax[0], minmax[1], nb) in fp32 (utils.py:1153), all on the device. */
+/* centers = tf.linspace(minmax[0], minmax[1], nb) in fp32 (utils.py:1153), all on the device; minmax = {min(x),
+ * max(x)} (K.min / K.max, utils.py:1151-1152) is nrt_item_stats_f32 with items = 1 and NRT_STAT_MINMAX. */
 NRT_API int nrt_mi_bin_centers_f32(const float* minmax, int nb, float* centers, void* stream);
 /* soft_quantize as a tensor op (utils.py:1099-1172): out[e*nb + b], e < n. */
 NRT_API int nrt_soft_quantize_f32(const float* x, int64_t n, const float* centers, int nb, float alpha, float min_clip,
@@ -285,12 +284,12 @@ NRT_API int nrt_philox_uniform_f32(uint64_t key, int64_t n, float lo, float hi, 
  * equal to shape's or 1 (broadcast).  x may be null and must not alias out. */
 NRT_API int nrt_philox_normal_f32(uint64_t key, const int32_t* shape, const int32_t* sd_shape, int ndim, const float* sd,
                           const float* sd_scale, const float* x, float* out, void* stream);
-/* Per-item statistics of x [items, n] in one pass: sums[item] = {sum d, sum d^2, max x, max |x|} (fp64,
- * d = x - x[item, 0]; may be null) and stat[item] (fp32; may be null) = kind 0: population SD
- * (tf.math.reduce_std), 1: max (reduce_max), 2: max |x|.  Deterministic: fixed-order block partials.
+/* Per-item reductions of x [items, n], deterministic (fixed-order block partials; the grid depends on (items, n)
+ * only).  SD: out[item] = population SD (fp64 sums of d = x - x[item, 0]; tf.math.reduce_std); MAX: max x;
+ * ABSMAX: max |x|; MINMAX: out[2 item] = min x, out[2 item + 1] = max x.  The extrema skip NaNs (fminf / fmaxf).
  * workspace: nrt_item_stats_workspace_bytes(items, n). */
 NRT_API int64_t nrt_item_stats_workspace_bytes(int items, int64_t n);
-NRT_API int nrt_item_stats_f32(const float* x, int items, int64_t n, int kind, double* sums, float* stat, void* workspace,
+NRT_API int nrt_item_stats_f32(const float* x, int items, int64_t n, int kind, float* out, void* workspace,
                        int64_t workspace_bytes, void* stream);
 /* Mean over Perlin levels: x [L, G, m] -> out [G, m],
  *   out[g, i] = (sum_l x[l, g, i] * divide_no_nan(before[l*G + g], after[l*G + g])) / L   (levels in order). */
@@ -320,13 +319,9 @@ NRT_API int nrt_labels_to_image_f32(const float* labels, int B, int64_t V, int C
                           const float* u, const float* mean_min, const float* mean_max, const float* bias,
                           int apply_exp, float* image, float* mean_out, float* bias_out, float* absmax,
                           void* workspace, int64_t workspace_bytes, void* stream);
-/* Per-item min and max of x [items, n]: mnmx[2 * item] = min, mnmx[2 * item + 1] = max (fixed-order block
- * partials).  workspace: nrt_item_minmax_workspace_bytes(items, n). */
-NRT_API int64_t nrt_item_minmax_workspace_bytes(int items, int64_t n);
-NRT_API int nrt_item_minmax_f32(const float* x, int items, int64_t n, float* mnmx, void* workspace,
-                          int64_t workspace_bytes, void* stream);
-/* x [items, n] with n = V * C -> out: y = x; with mnmx, y = div_no_nan(y - mn, mx - mn); with gamma_u [items, C],
- * y = powf(y, gamma_u[item, c] * (gamma_hi - gamma_lo) + gamma_lo).  out must not alias x. */
+/* x [items, n] with n = V * C -> out: y = x; with mnmx (the NRT_STAT_MINMAX output of nrt_item_stats_f32),
+ * y = div_no_nan(y - mn, mx - mn); with gamma_u [items, C], y = powf(y, gamma_u[item, c] * (gamma_hi - gamma_lo) +
+ * gamma_lo).  out must not alias x. */
 NRT_API int nrt_norm_gamma_f32(const float* x, int items, int64_t n, int C, const float* mnmx, const float* gamma_u,
                           float gamma_lo, float gamma_hi, float* out, void* stream);
 /* Output label map: l = crop(label), then l = lut[l] when lut is non-null.  _f32 writes the one-hot out [B, V, M]

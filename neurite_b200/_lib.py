@@ -72,8 +72,6 @@ SIGNATURES = {
                                        ctypes.c_int, ctypes.c_int, c_i64, c_f32, c_f32, c_f32,
                                        c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]),
     'nrt_mi_minmax_bwd_f32': (ctypes.c_int, [c_vp, c_i64, c_vp, c_vp, ctypes.c_int, c_vp, c_vp]),
-    'nrt_minmax_workspace_bytes': (c_i64, []),
-    'nrt_minmax_f32': (ctypes.c_int, [c_vp, c_i64, c_vp, c_vp, c_i64, c_vp]),
     'nrt_mi_bin_centers_f32': (ctypes.c_int, [c_vp, ctypes.c_int, c_vp, c_vp]),
     'nrt_soft_quantize_f32': (ctypes.c_int, [c_vp, c_i64, c_vp, ctypes.c_int, c_f32, c_f32, c_f32,
                                               ctypes.c_int, c_vp, c_vp]),
@@ -83,7 +81,7 @@ SIGNATURES = {
     'nrt_philox_uniform_f32': (ctypes.c_int, [c_u64, c_i64, c_f32, c_f32, c_vp, c_vp]),
     'nrt_philox_normal_f32': (ctypes.c_int, [c_u64, P_I32, P_I32, ctypes.c_int, c_vp, c_vp, c_vp, c_vp, c_vp]),
     'nrt_item_stats_workspace_bytes': (c_i64, [ctypes.c_int, c_i64]),
-    'nrt_item_stats_f32': (ctypes.c_int, [c_vp, ctypes.c_int, c_i64, ctypes.c_int, c_vp, c_vp, c_vp, c_i64, c_vp]),
+    'nrt_item_stats_f32': (ctypes.c_int, [c_vp, ctypes.c_int, c_i64, ctypes.c_int, c_vp, c_vp, c_i64, c_vp]),
     'nrt_level_combine_f32': (ctypes.c_int, [c_vp, ctypes.c_int, ctypes.c_int, c_i64, c_vp, c_vp, c_vp, c_vp]),
     'nrt_philox_normal_background_f32': (ctypes.c_int, [c_u64, ctypes.c_int, c_i64, ctypes.c_int, c_vp, c_vp, c_vp,
                                                          c_vp, c_i64, c_i64, c_i64, c_i64, c_vp, c_f32, c_vp, c_vp]),
@@ -91,8 +89,6 @@ SIGNATURES = {
     'nrt_labels_to_image_f32': (ctypes.c_int, [c_vp, ctypes.c_int, c_i64, ctypes.c_int, c_i64, c_i64, c_i64, c_i64,
                                                 c_vp, ctypes.c_int, ctypes.c_int, c_vp, c_vp, c_vp, c_vp, ctypes.c_int,
                                                 c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]),
-    'nrt_item_minmax_workspace_bytes': (c_i64, [ctypes.c_int, c_i64]),
-    'nrt_item_minmax_f32': (ctypes.c_int, [c_vp, ctypes.c_int, c_i64, c_vp, c_vp, c_i64, c_vp]),
     'nrt_norm_gamma_f32': (ctypes.c_int, [c_vp, ctypes.c_int, c_i64, ctypes.c_int, c_vp, c_vp, c_f32, c_f32, c_vp,
                                            c_vp]),
     'nrt_label_map_f32': (ctypes.c_int, [c_vp, ctypes.c_int, c_i64, c_i64, c_i64, c_i64, c_i64, c_vp, ctypes.c_int,
@@ -120,14 +116,15 @@ def _load():
         fn = getattr(lib, name)          # AttributeError if the header and the library diverge
         fn.restype = res
         fn.argtypes = args
-    if lib.nrt_version() != 1:
-        raise ImportError('neurite_b200: ABI version mismatch (library %d, binding 1)' % lib.nrt_version())
+    if lib.nrt_version() != 2:
+        raise ImportError('neurite_b200: ABI version mismatch (library %d, binding 2)' % lib.nrt_version())
     return lib
 
 
 lib = _load()
 
 NRT_LINEAR, NRT_NEAREST = 0, 1
+NRT_STAT_SD, NRT_STAT_MAX, NRT_STAT_ABSMAX, NRT_STAT_MINMAX = 0, 1, 2, 3
 ACTIVATIONS = {None: 0, 'linear': 0, 'relu': 1, 'sigmoid': 2, 'tanh': 3}
 
 

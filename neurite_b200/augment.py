@@ -24,10 +24,10 @@ import numpy as np
 import torch
 
 from . import utils
-from ._lib import lib, check, ptr, stream_ptr, i32_array, require_cuda
+from ._lib import lib, check, ptr, stream_ptr, i32_array, require_cuda, NRT_STAT_SD, NRT_STAT_MAX
 
 _MAX_SEED = np.iinfo(int).max
-_STAT_KIND = {'std': 0, 'max': 1}
+_STAT_KIND = {'std': NRT_STAT_SD, 'max': NRT_STAT_MAX}
 
 
 def normalize_axes(axes, shape, allowed=None, none_means_all=False):
@@ -78,18 +78,6 @@ def _draw_sigmas(rand, std_min, std_max, n_dim, isotropic):
     return sig[:1] * n_dim if isotropic else sig
 
 
-def _item_stats(x2d, kind, out=None):
-    """fp32 statistic of every row of the contiguous fp32 [items, n] view x2d, on the device."""
-    items, n = x2d.shape
-    stat = torch.empty(items, dtype=torch.float32, device=x2d.device) if out is None else out
-    nb = lib.nrt_item_stats_workspace_bytes(int(items), int(n))
-    ws = utils._scratch(x2d.device, nb)
-    with torch.cuda.device(x2d.device):
-        check(lib.nrt_item_stats_f32(ptr(x2d), int(items), int(n), int(kind), None, ptr(stat), ptr(ws), nb,
-                                     stream_ptr(x2d.device)))
-    return stat
-
-
 def _draw_perlin_full_from_draws(noise, sigmas, std_max, reduce='std'):
     """The deterministic rest of draw_perlin_full once the draws are made.
 
@@ -111,7 +99,7 @@ def _draw_perlin_full_from_draws(noise, sigmas, std_max, reduce='std'):
 
     def stats(t):
         if kind is not None:
-            return _item_stats(t.reshape(L * G, m), kind)
+            return utils._item_stats(t.reshape(L * G, m), kind)
         return torch.stack([torch.as_tensor(reduce(t[l, g]), device=dev).reshape(())
                             for l in range(L) for g in range(G)]).to(torch.float32)
 

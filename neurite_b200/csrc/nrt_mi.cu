@@ -478,59 +478,6 @@ __global__ void mi_finalize_kernel(const float* stats, int nbx, int nby, float e
   if (threadIdx.x == 0) mi[item] = (float)tot;
 }
 
-// ---- min / max of a tensor (bin centres default to linspace(min, max), utils.py:1151-1153) ----
-constexpr int kMmBlocks = 1024;
-__global__ void __launch_bounds__(256) minmax_partial_kernel(const float* x, int64_t n, float* partial) {
-  float mn = INFINITY, mx = -INFINITY;
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if ((reinterpret_cast<uintptr_t>(x) & 15u) == 0) {
-    const float4* x4 = reinterpret_cast<const float4*>(x);
-    const int64_t n4 = n >> 2;
-    for (int64_t i = tid; i < n4; i += stride) {
-      const float4 v = ld_stream_f4(x4 + i);
-      mn = fminf(fminf(mn, v.x), fminf(v.y, fminf(v.z, v.w)));
-      mx = fmaxf(fmaxf(mx, v.x), fmaxf(v.y, fmaxf(v.z, v.w)));
-    }
-    for (int64_t i = (n4 << 2) + tid; i < n; i += stride) {
-      mn = fminf(mn, x[i]);
-      mx = fmaxf(mx, x[i]);
-    }
-  } else {
-    for (int64_t i = tid; i < n; i += stride) {
-      mn = fminf(mn, x[i]);
-      mx = fmaxf(mx, x[i]);
-    }
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, o));
-    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-  }
-  __shared__ float smn[8], smx[8];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (lane == 0) { smn[warp] = mn; smx[warp] = mx; }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    for (int w = 1; w < 8; ++w) { mn = fminf(mn, smn[w]); mx = fmaxf(mx, smx[w]); }
-    partial[2 * blockIdx.x] = mn;
-    partial[2 * blockIdx.x + 1] = mx;
-  }
-}
-__global__ void minmax_final_kernel(const float* partial, int nblk, float* out2) {
-  float mn = INFINITY, mx = -INFINITY;
-  for (int i = threadIdx.x; i < nblk; i += 32) {
-    mn = fminf(mn, partial[2 * i]);
-    mx = fmaxf(mx, partial[2 * i + 1]);
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, o));
-    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-  }
-  if (threadIdx.x == 0) { out2[0] = mn; out2[1] = mx; }
-}
-
 // tf.linspace(min, max, nb) in fp32: endpoints exact, interior start + delta * i
 __global__ void mi_centers_kernel(const float* minmax, int nb, float* centers) {
   const int i = threadIdx.x;
@@ -639,22 +586,6 @@ int nrt_mi_finalize_f32(const float* stats, int items, int nbx, int nby, float e
   NRT_REQUIRE(items >= 1 && nbx >= 1 && nby >= 1, NRT_E_ARG, "bad items/bins");
   mi_finalize_kernel<<<items, 128, 0, static_cast<cudaStream_t>(stream)>>>(stats, nbx, nby, eps, mi);
   return check_launch("mi_finalize_kernel");
-}
-
-int64_t nrt_minmax_workspace_bytes(void) { return (int64_t)kMmBlocks * 2 * sizeof(float); }
-
-int nrt_minmax_f32(const float* x, int64_t n, float* out2, void* workspace, int64_t workspace_bytes, void* stream) {
-  NRT_REQUIRE(x && out2 && workspace, NRT_E_ARG, "null pointer");
-  NRT_REQUIRE(n >= 1, NRT_E_ARG, "min/max of an empty tensor");
-  NRT_REQUIRE(workspace_bytes >= nrt_minmax_workspace_bytes(), NRT_E_ARG, "workspace too small");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  int nblk = (int)imin64((n / 4 + 255) / 256, kMmBlocks);
-  if (nblk < 1) nblk = 1;
-  minmax_partial_kernel<<<nblk, 256, 0, st>>>(x, n, static_cast<float*>(workspace));
-  int rc = check_launch("minmax_partial_kernel");
-  if (rc != NRT_OK) return rc;
-  minmax_final_kernel<<<1, 32, 0, st>>>(static_cast<const float*>(workspace), nblk, out2);
-  return check_launch("minmax_final_kernel");
 }
 
 int nrt_mi_bin_centers_f32(const float* minmax, int nb, float* centers, void* stream) {

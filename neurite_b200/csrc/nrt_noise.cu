@@ -1,5 +1,6 @@
 // nrt_noise.cu -- the noise fields of the synthesis generator: a counter-based Philox4x32-10 stream (uniform SD
-// tables, normal noise scaled by a broadcast SD table), per-item statistics and the mean over Perlin levels.
+// tables, normal noise scaled by a broadcast SD table) and the mean over Perlin levels.  The per-item statistics
+// the fields are rescaled by are in nrt_stats.cu.
 //
 // Reference: neurite/tf/utils/augment.py:65-218 (random_blur_rescale, draw_perlin_full), neurite/tf/layers.py:
 // 2305-2508 (GaussianNoise, PerlinNoise).  TF's random stream cannot be reproduced outside TF; this one is defined
@@ -148,92 +149,6 @@ __global__ void __launch_bounds__(256) philox_normal_background_kernel(
   }
 }
 
-// ---- per-item statistics: [items, n] -> {sum d, sum d^2, max x, max |x|} with d = x - x[item, 0] ----
-// The shift by the item's first element makes the variance of a constant item exactly 0.  Every block writes
-// one partial per item, the final kernel adds the partials of an item in a fixed order: deterministic.
-constexpr int kStatThreads = 256;
-constexpr int kStatMaxBlocks = 256;
-
-inline int stat_blocks(int64_t n) {
-  const int64_t b = (n + 16383) / 16384;
-  return (int)(b < 1 ? 1 : (b > kStatMaxBlocks ? kStatMaxBlocks : b));
-}
-
-__global__ void __launch_bounds__(kStatThreads) item_stats_partial_kernel(const float* __restrict__ x, int64_t n,
-                                                                          double* __restrict__ partial) {
-  const int nbx = gridDim.x, item = blockIdx.y;
-  const float* xi = x + (int64_t)item * n;
-  const float shift = __ldg(xi);
-  const int64_t chunk = (n + nbx - 1) / nbx;
-  const int64_t e0 = (int64_t)blockIdx.x * chunk;
-  const int64_t e1 = e0 + chunk < n ? e0 + chunk : n;
-  double s1 = 0.0, s2 = 0.0;
-  float mx = -INFINITY, mxa = 0.f;
-  for (int64_t e = e0 + threadIdx.x; e < e1; e += kStatThreads) {
-    const float v = ld_stream_f(xi + e);
-    const double d = (double)v - (double)shift;
-    s1 += d;
-    s2 = fma(d, d, s2);
-    mx = fmaxf(mx, v);
-    mxa = fmaxf(mxa, fabsf(v));
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    s1 += __shfl_xor_sync(0xffffffffu, s1, o);
-    s2 += __shfl_xor_sync(0xffffffffu, s2, o);
-    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-    mxa = fmaxf(mxa, __shfl_xor_sync(0xffffffffu, mxa, o));
-  }
-  __shared__ double sh[kStatThreads / 32][4];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (lane == 0) { sh[warp][0] = s1; sh[warp][1] = s2; sh[warp][2] = mx; sh[warp][3] = mxa; }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    for (int w = 1; w < kStatThreads / 32; ++w) {
-      s1 += sh[w][0]; s2 += sh[w][1];
-      mx = fmaxf(mx, (float)sh[w][2]); mxa = fmaxf(mxa, (float)sh[w][3]);
-    }
-    double* p = partial + ((int64_t)item * nbx + blockIdx.x) * 4;
-    p[0] = s1; p[1] = s2; p[2] = mx; p[3] = mxa;
-  }
-}
-
-// one warp per item; kind 0: population SD (tf.math.reduce_std), 1: max (reduce_max), 2: max |x|
-__global__ void item_stats_final_kernel(const double* __restrict__ partial, int nbx, int64_t n, int kind,
-                                        double* __restrict__ sums, float* __restrict__ stat) {
-  const int item = blockIdx.x, lane = threadIdx.x;
-  double s1 = 0.0, s2 = 0.0;
-  float mx = -INFINITY, mxa = 0.f;
-  for (int b = lane; b < nbx; b += 32) {
-    const double* p = partial + ((int64_t)item * nbx + b) * 4;
-    s1 += p[0]; s2 += p[1];
-    mx = fmaxf(mx, (float)p[2]); mxa = fmaxf(mxa, (float)p[3]);
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    s1 += __shfl_xor_sync(0xffffffffu, s1, o);
-    s2 += __shfl_xor_sync(0xffffffffu, s2, o);
-    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-    mxa = fmaxf(mxa, __shfl_xor_sync(0xffffffffu, mxa, o));
-  }
-  if (lane != 0) return;
-  if (sums) {
-    double* s = sums + (int64_t)item * 4;
-    s[0] = s1; s[1] = s2; s[2] = mx; s[3] = mxa;
-  }
-  if (stat) {
-    float r;
-    if (kind == 0) {
-      const double m = s1 / (double)n;
-      const double var = s2 / (double)n - m * m;
-      r = (float)sqrt(var > 0.0 ? var : 0.0);
-    } else {
-      r = kind == 1 ? mx : mxa;
-    }
-    stat[item] = r;
-  }
-}
-
 // out[g, i] = (sum_l x[l, g, i] * divide_no_nan(before[l*G + g], after[l*G + g])) / L, levels in order
 __global__ void __launch_bounds__(256) level_combine_kernel(const float* __restrict__ x, int L, int G, int64_t m,
                                                             const float* __restrict__ before,
@@ -327,27 +242,6 @@ int nrt_philox_normal_background_f32(uint64_t key, int B, int64_t V, int C, cons
       (uint32_t)key, (uint32_t)(key >> 32), (uint32_t)V, (uint32_t)C, (uint32_t)n, sd, sd_scale, x, labels,
       (uint32_t)crop_L, (uint32_t)crop_inner, (uint32_t)crop_lo, (uint32_t)crop_hi, bg_u, zero_background, out);
   return check_launch("philox_normal_background_kernel");
-}
-
-int64_t nrt_item_stats_workspace_bytes(int items, int64_t n) {
-  return (int64_t)items * stat_blocks(n) * 4 * (int64_t)sizeof(double);
-}
-
-int nrt_item_stats_f32(const float* x, int items, int64_t n, int kind, double* sums, float* stat, void* workspace,
-                       int64_t workspace_bytes, void* stream) {
-  NRT_REQUIRE(x && workspace && (sums || stat), NRT_E_ARG, "null pointer");
-  NRT_REQUIRE(items >= 1 && items <= 65535, NRT_E_ARG, "items = %d outside 1..65535", items);
-  NRT_REQUIRE(n >= 1, NRT_E_ARG, "statistics of an empty item");
-  NRT_REQUIRE(kind >= 0 && kind <= 2, NRT_E_ARG, "kind = %d outside 0..2", kind);
-  NRT_REQUIRE(workspace_bytes >= nrt_item_stats_workspace_bytes(items, n), NRT_E_ARG, "workspace too small");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int nbx = stat_blocks(n);
-  double* partial = static_cast<double*>(workspace);
-  item_stats_partial_kernel<<<dim3(nbx, items), kStatThreads, 0, st>>>(x, n, partial);
-  int rc = check_launch("item_stats_partial_kernel");
-  if (rc) return rc;
-  item_stats_final_kernel<<<items, 32, 0, st>>>(partial, nbx, n, kind, sums, stat);
-  return check_launch("item_stats_final_kernel");
 }
 
 int nrt_level_combine_f32(const float* x, int L, int G, int64_t m, const float* before, const float* after,

@@ -1,6 +1,6 @@
 // nrt_synth.cu -- the label-to-image stages of the synthesis generator labels_to_image_new: per-label intensities
-// with the bias field, per-item min/max with min-max normalisation and gamma, the output label map (one-hot or
-// remapped) and the crop window of RandomCrop.
+// with the bias field, min-max normalisation and gamma, the output label map (one-hot or remapped) and the crop
+// window of RandomCrop.
 //
 // Reference: neurite/tf/models.py:1162-1282 (labels_to_image_new), neurite/tf/layers.py:446-519 (RandomCrop),
 // neurite/tf/utils/utils.py:953-968 (minmax_norm).
@@ -95,62 +95,7 @@ __global__ void absmax_final_kernel(const float* __restrict__ partial, int nb, f
   if (threadIdx.x == 0) *out = m;
 }
 
-// ---- 3: per-item min / max, then (x - mn) / (mx - mn) and / or the gamma power ----
-constexpr int kMmThreads = 256;
-constexpr int kMmMaxBlocks = 1024;
-
-// enough blocks per item to fill every SM ~8 times over the whole batch, at least 4096 elements per block
-inline int mm_blocks(int items, int64_t n) {
-  const int64_t want = ((int64_t)sm_count() * 8 + items - 1) / items;
-  const int64_t cap = (n + 4095) / 4096;
-  const int64_t b = want < cap ? want : cap;
-  return (int)(b < 1 ? 1 : (b > kMmMaxBlocks ? kMmMaxBlocks : b));
-}
-
-__global__ void __launch_bounds__(kMmThreads) item_minmax_partial_kernel(const float* __restrict__ x, int64_t n,
-                                                                          float2* __restrict__ partial) {
-  const int nbx = gridDim.x, item = blockIdx.y;
-  const float* xi = x + (int64_t)item * n;
-  const int64_t chunk = (n + nbx - 1) / nbx;
-  const int64_t e0 = (int64_t)blockIdx.x * chunk;
-  const int64_t e1 = e0 + chunk < n ? e0 + chunk : n;
-  float mn = INFINITY, mx = -INFINITY;
-  for (int64_t e = e0 + threadIdx.x; e < e1; e += kMmThreads) {
-    const float v = ld_stream_f(xi + e);
-    mn = fminf(mn, v);
-    mx = fmaxf(mx, v);
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, o));
-    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-  }
-  __shared__ float2 sh[kMmThreads / 32];
-  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = make_float2(mn, mx);
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    for (int i = 1; i < kMmThreads / 32; ++i) { mn = fminf(mn, sh[i].x); mx = fmaxf(mx, sh[i].y); }
-    partial[(int64_t)item * nbx + blockIdx.x] = make_float2(mn, mx);
-  }
-}
-
-// one warp per item: mnmx[item] = {min, max}
-__global__ void item_minmax_final_kernel(const float2* __restrict__ partial, int nbx, float2* __restrict__ mnmx) {
-  const int item = blockIdx.x;
-  float mn = INFINITY, mx = -INFINITY;
-  for (int b = threadIdx.x; b < nbx; b += 32) {
-    const float2 p = partial[(int64_t)item * nbx + b];
-    mn = fminf(mn, p.x);
-    mx = fmaxf(mx, p.y);
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, o));
-    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-  }
-  if (threadIdx.x == 0) mnmx[item] = make_float2(mn, mx);
-}
-
+// ---- 3: (x - mn) / (mx - mn) with the per-item min / max of nrt_stats.cu, and / or the gamma power ----
 __global__ void __launch_bounds__(256) norm_gamma_kernel(const float* __restrict__ x, int items, int64_t n, int C,
                                                          const float2* __restrict__ mnmx,
                                                          const float* __restrict__ gamma_u, float g_lo, float g_hi,
@@ -281,25 +226,6 @@ int nrt_labels_to_image_f32(const float* labels, int B, int64_t V, int C, int64_
   if (int rc = check_launch("labels_to_image_kernel")) return rc;
   absmax_final_kernel<<<1, 32, 0, st>>>(partial, nb, absmax);
   return check_launch("absmax_final_kernel");
-}
-
-int64_t nrt_item_minmax_workspace_bytes(int items, int64_t n) {
-  return (int64_t)items * mm_blocks(items, n) * (int64_t)sizeof(float2);
-}
-
-int nrt_item_minmax_f32(const float* x, int items, int64_t n, float* mnmx, void* workspace, int64_t workspace_bytes,
-                        void* stream) {
-  NRT_REQUIRE(x && mnmx && workspace, NRT_E_ARG, "null pointer");
-  NRT_REQUIRE(items >= 1 && items <= 65535, NRT_E_ARG, "items = %d outside 1..65535", items);
-  NRT_REQUIRE(n >= 1, NRT_E_ARG, "min / max of an empty item");
-  NRT_REQUIRE(workspace_bytes >= nrt_item_minmax_workspace_bytes(items, n), NRT_E_ARG, "workspace too small");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int nbx = mm_blocks(items, n);
-  float2* partial = static_cast<float2*>(workspace);
-  item_minmax_partial_kernel<<<dim3(nbx, items), kMmThreads, 0, st>>>(x, n, partial);
-  if (int rc = check_launch("item_minmax_partial_kernel")) return rc;
-  item_minmax_final_kernel<<<items, 32, 0, st>>>(partial, nbx, reinterpret_cast<float2*>(mnmx));
-  return check_launch("item_minmax_final_kernel");
 }
 
 int nrt_norm_gamma_f32(const float* x, int items, int64_t n, int C, const float* mnmx, const float* gamma_u,

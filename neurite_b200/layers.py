@@ -867,7 +867,7 @@ class GaussianNoise(_Layer):
             check(lib.nrt_philox_uniform_f32(k_sd, n_sd, float(self.noise_min), float(self.noise_max), ptr(table),
                                              st))
             if not self.absolute and x32.numel():
-                scale = augment._item_stats(x32.detach().reshape(1, -1), 2)
+                scale = utils._item_stats(x32.detach().reshape(1, -1), _lib.NRT_STAT_ABSMAX)
         if self.noise_only:
             out = torch.empty_like(x32, memory_format=torch.contiguous_format)
             with torch.cuda.device(x.device):

@@ -13,7 +13,7 @@ Stages and where they run:
     crop, generation LUT, per-label means, exp(bias), max |image|     nrt_labels_to_image_f32 (one pass)
     GaussianNoise (+ background clearing)     nrt_philox_normal_f32 / nrt_philox_normal_background_f32
     random GaussianBlur, Subsample            utils.separable_conv, utils.gather_axis
-    per-item min / max, normalisation, gamma  nrt_item_minmax_f32, nrt_norm_gamma_f32
+    per-item min / max, normalisation, gamma  nrt_item_stats_f32, nrt_norm_gamma_f32
     crop, output LUT, one-hot / int map       nrt_label_map_f32 / nrt_label_map_i32
 
 Randomness.  Every component (shift, rot, scale, shear, flip, swap, warp, crop, mean, bias, noise, background,
@@ -36,7 +36,7 @@ input_model raises NotImplementedError.
 import numpy as np
 import torch
 
-from . import augment, layers, utils
+from . import _lib, augment, layers, utils
 from ._lib import lib, check, ptr, stream_ptr, i32_array, require_cuda
 
 _MAX_SEED = np.iinfo(int).max
@@ -398,7 +398,7 @@ class LabelsToImage(torch.nn.Module):
 
         if c['normalize'] or plan['gamma_u'] is not None:
             x2d = image.contiguous().reshape(B, -1)
-            mnmx = utils._item_minmax(x2d) if c['normalize'] else None
+            mnmx = utils._item_stats(x2d, _lib.NRT_STAT_MINMAX) if c['normalize'] else None
             image = utils._norm_gamma(x2d, C, mnmx, plan['gamma_u'], c['gamma']).reshape(image.shape)
 
         # output label map

@@ -448,16 +448,24 @@ def _scratch(device, nbytes):
     return _stream_scratch(_SCRATCH, 8, device, nbytes)
 
 
+def _item_stats(x2d, kind):
+    """Per-row reduction of the contiguous fp32 [items, n] view x2d on the device (nrt_item_stats_f32): [items] for
+    NRT_STAT_SD / MAX / ABSMAX, [items, 2] = (min, max) for NRT_STAT_MINMAX."""
+    items, n = x2d.shape
+    out = torch.empty((items, 2) if kind == _lib.NRT_STAT_MINMAX else (items,), dtype=torch.float32, device=x2d.device)
+    nb = lib.nrt_item_stats_workspace_bytes(int(items), int(n))
+    ws = _scratch(x2d.device, nb)
+    with torch.cuda.device(x2d.device):
+        check(lib.nrt_item_stats_f32(ptr(x2d), int(items), int(n), int(kind), ptr(out), ptr(ws), nb,
+                                     stream_ptr(x2d.device)))
+    return out
+
+
 def minmax(x, group=None):
     """device tensor [min(x), max(x)] (K.min / K.max, utils.py:1151-1152), no host sync.
     With `group`, the extrema over every rank's shard (one MIN all-reduce of [min, -max])."""
     require_cuda(x)
-    x32 = _as_f32(x).contiguous()
-    out = torch.empty(2, dtype=torch.float32, device=x.device)
-    nb = lib.nrt_minmax_workspace_bytes()
-    ws = _scratch(x.device, nb)
-    with torch.cuda.device(x.device):
-        check(lib.nrt_minmax_f32(ptr(x32), x32.numel(), ptr(out), ptr(ws), nb, stream_ptr(x.device)))
+    out = _item_stats(_as_f32(x).contiguous().reshape(1, -1), _lib.NRT_STAT_MINMAX).reshape(2)
     if group is not None:
         import torch.distributed as dist
         packed = torch.stack([out[0], -out[1]])
@@ -684,17 +692,6 @@ def subsample_axis(x, stride_min=1, stride_max=8, axes=None, prob=1, upsample=Tr
     return gather_axis(x, subsample_indices(x.shape[ax], thick, upsample), ax)
 
 
-def _item_minmax(x2d):
-    """device [items, 2] = per-row (min, max) of the contiguous fp32 [items, n] view x2d (nrt_item_minmax_f32)."""
-    items, n = x2d.shape
-    mnmx = torch.empty(items, 2, dtype=torch.float32, device=x2d.device)
-    nb = lib.nrt_item_minmax_workspace_bytes(int(items), int(n))
-    ws = _scratch(x2d.device, nb)
-    with torch.cuda.device(x2d.device):
-        check(lib.nrt_item_minmax_f32(ptr(x2d), int(items), int(n), ptr(mnmx), ptr(ws), nb, stream_ptr(x2d.device)))
-    return mnmx
-
-
 def _norm_gamma(x2d, C, mnmx, gamma_u=None, gamma=0.0):
     """[items, n] -> div_no_nan(x - mn, mx - mn) per row (mnmx may be None: no normalisation), then
     pow(., u * (2 gamma) + (1 - gamma)) with gamma_u [items, C] when given (nrt_norm_gamma_f32)."""
@@ -730,7 +727,7 @@ def minmax_norm(x, axis=None):
     if x32.numel() == 0:
         return x32.clone()
     x2d = x32.reshape(items, n)
-    out = _norm_gamma(x2d, 1, _item_minmax(x2d)).reshape(x32.shape)
+    out = _norm_gamma(x2d, 1, _item_stats(x2d, _lib.NRT_STAT_MINMAX)).reshape(x32.shape)
     return out.to(x.dtype) if x.dtype.is_floating_point and x.dtype != torch.float32 else out
 
 

@@ -23,7 +23,7 @@ def declared_symbols():
     return sorted(set(re.findall(r'\b(nrt_[a-z0-9_]+)\s*\(', src)))
 
 
-def test_library_loads_and_exports_every_declared_symbol():
+def test_library_loads_at_abi_version_2_and_exports_every_declared_symbol():
     from neurite_b200 import _lib
     names = declared_symbols()
     assert len(names) >= 14
@@ -31,11 +31,11 @@ def test_library_loads_and_exports_every_declared_symbol():
     for n in names:
         assert hasattr(raw, n), 'libneurite_b200.so does not export %s' % n
     assert sorted(_lib.SIGNATURES) == names, 'ctypes binding and header diverge'
-    assert _lib.lib.nrt_version() == 1
+    assert _lib.lib.nrt_version() == 2
     assert _lib.lib.nrt_status_string(0) == b'ok'
 
 
-def test_argument_validation_returns_status_codes():
+def test_entry_points_return_status_codes_on_bad_arguments():
     from neurite_b200 import _lib
     lib = _lib.lib
     null = ctypes.c_void_p(0)
@@ -72,7 +72,7 @@ def test_argument_validation_returns_status_codes():
                               one, one, one, null, null, 0, null) == -2                                 # gradient: <= 32 bins
     assert lib.nrt_mi_bwd_f32(one, 1, 1, 1, 16, one, one, 1, 1, 1, 16, one, 1, 1, 10, f(1.0), f(-inf), f(inf),
                               one, null, null, null, null, 0, null) == -1                               # no gradient requested
-    assert lib.nrt_minmax_f32(one, 0, one, one, 1 << 20, null) == -1                                    # empty tensor
+    assert lib.nrt_item_stats_f32(one, 1, 0, _lib.NRT_STAT_MINMAX, one, one, 1 << 20, null) == -1         # empty tensor
     assert lib.nrt_sepconv_axis_f32(one, one, 1, 8, 1, one, 3, 1, 1, 1, 8, null) == -1                  # in place
     assert b'in-place' in lib.nrt_last_error_string()
     two = ctypes.c_void_p(32)

@@ -141,17 +141,26 @@ def test_items_and_levels_are_independent(ne):
 
 
 # ------------------------------------------------------------------ statistics
-def test_item_stats_against_fp64(ne):
+def test_item_stats_every_kind_against_numpy_and_fp64(ne):
+    """Every kind of nrt_item_stats_f32: odd n with several items (rows alternate between float4 and scalar
+    loads), n = 1, a base one float past an aligned allocation, and one item large enough to reach the grid cap."""
+    L = ne._lib
+    stats = ne.utils._item_stats
     rng = np.random.default_rng(3)
-    for items, n in ((3, 100001), (1, 7), (5, 4097)):
+    for items, n, offset in ((3, 100001, 0), (1, 7, 0), (5, 4097, 0), (4, 1, 0), (3, 1027, 1), (1, 5000003, 0)):
         x = (rng.standard_normal((items, n)) * 3 + 5).astype(F32)
-        xd = dev(x)
-        x64 = x.astype(np.float64)
-        for kind, ref in ((0, x64.std(1)), (1, x64.max(1)), (2, np.abs(x64).max(1))):
-            got = ne.augment._item_stats(xd, kind).cpu().numpy()
-            np.testing.assert_allclose(got, ref, rtol=2 * U, atol=0)
+        buf = torch.empty(items * n + offset, device='cuda')
+        xd = buf[offset:].view(items, n)
+        xd.copy_(torch.from_numpy(x))
+        sd = stats(xd, L.NRT_STAT_SD).cpu().numpy()
+        np.testing.assert_allclose(sd, x.astype(np.float64).std(1), rtol=2 * U, atol=0)
+        assert np.array_equal(stats(xd, L.NRT_STAT_MAX).cpu().numpy(), x.max(1))
+        assert np.array_equal(stats(xd, L.NRT_STAT_ABSMAX).cpu().numpy(), np.abs(x).max(1))
+        assert np.array_equal(stats(xd, L.NRT_STAT_MINMAX).cpu().numpy(), np.stack([x.min(1), x.max(1)], 1))
+        if offset:                                   # the summation order does not depend on the address
+            assert np.array_equal(stats(dev(x), L.NRT_STAT_SD).cpu().numpy(), sd)
     c = dev(np.full((2, 12345), 0.1, F32))
-    assert torch.equal(ne.augment._item_stats(c, 0).cpu(), torch.zeros(2))
+    assert torch.equal(stats(c, L.NRT_STAT_SD).cpu(), torch.zeros(2))
 
 
 def test_constant_input_gives_zero(ne):
@@ -223,10 +232,11 @@ def test_profiler_no_device_to_host_copy(ne):
     if not any('kernel' in n for n in names):
         pytest.skip('torch.profiler recorded no CUDA kernels on this machine')
     assert not any('DtoH' in n or 'DeviceToHost' in n for n in names), [n for n in names if 'DtoH' in n]
-    # PerlinNoise: the draws, the blur passes, the statistics and the level mean; GaussianNoise: the SD table,
-    # max|x| and the fused x + noise pass (philox_uniform / philox_normal / item_stats_*)
-    for k in ('philox_uniform_kernel', 'philox_normal_kernel', 'item_stats_partial_kernel',
-              'item_stats_final_kernel', 'level_combine_kernel', 'sepconv_'):
+    # PerlinNoise: the draws, the blur passes, the SDs and the level mean; GaussianNoise: the SD table, max|x| and
+    # the fused x + noise pass (philox_uniform / philox_normal / item_stats_*<true> for SD, <false> for max|x|)
+    for k in ('philox_uniform_kernel', 'philox_normal_kernel', 'item_stats_partial_kernel<true>',
+              'item_stats_final_kernel<true>', 'item_stats_partial_kernel<false>', 'item_stats_final_kernel<false>',
+              'level_combine_kernel', 'sepconv_'):
         assert any(k in n for n in names), k
 
 

@@ -119,12 +119,12 @@ def test_noise_background_matches_normal_kernel(B, shape, C):
 
 @pytest.mark.parametrize('B,n,C', [(1, 7, 1), (2, 1023, 3), (3, 40001, 2), (1, 1, 1)])
 @pytest.mark.parametrize('gamma', [0.0, 0.5])
-def test_minmax_norm_gamma_kernels(B, n, C, gamma):
+def test_item_stats_minmax_then_norm_gamma_kernels(B, n, C, gamma):
     rng = np.random.default_rng(n)
     x = rng.normal(0, 3, (B, n * C)).astype(F32)
     gu = rng.random((B, C), dtype=F32) if gamma else None
     xd = _t(x)
-    mnmx = ne.utils._item_minmax(xd)
+    mnmx = ne.utils._item_stats(xd, ne._lib.NRT_STAT_MINMAX)
     assert np.array_equal(mnmx.cpu().numpy(), np.stack([x.min(1), x.max(1)], 1))
     d_gu = None if gu is None else _t(gu)
     out = ne.utils._norm_gamma(xd, C, mnmx, d_gu, gamma).cpu().numpy()
@@ -303,14 +303,15 @@ def _kernel_names(fn):
     return names
 
 
-def test_profiler_kernels_and_no_device_to_host_copy():
+def test_profiler_generator_kernels_and_no_device_to_host_copy():
     gen = ne.models.labels_to_image_new(range(8), in_shape=(16, 16, 16), zero_background=1, seeds={'mean': 1})
     x = _label_input(np.random.default_rng(4), 2, (16, 16, 16), range(8))
     gen(x)
     torch.cuda.synchronize()
     names = _kernel_names(lambda: gen(x))
     for k in ('labels_to_image_kernel', 'absmax_final_kernel', 'philox_normal_background_kernel',
-              'item_minmax_partial_kernel', 'item_minmax_final_kernel', 'norm_gamma_kernel', 'one_hot_kernel'):
+              'item_stats_partial_kernel<false>', 'item_stats_final_kernel<false>', 'norm_gamma_kernel',
+              'one_hot_kernel'):
         assert any(k in n for n in names), k
     assert not any('DtoH' in n or 'Device -> Host' in n for n in names), [n for n in names if 'Memcpy' in n]
     gen_i = ne.models.labels_to_image_new(range(8), in_shape=(16, 16, 16), one_hot=False, labels_out={1: 1, 2: 5})

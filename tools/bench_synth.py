@@ -81,7 +81,7 @@ def bench(M, iters, warmup):
     gu = plan['gamma_u']
 
     def k3():
-        mm = ne.utils._item_minmax(x2d)
+        mm = ne.utils._item_stats(x2d, ne._lib.NRT_STAT_MINMAX)
         return ne.utils._norm_gamma(x2d, 1, mm, gu, 0.5)
     out.append(rec('3 min/max + normalise + gamma (two reads, one write)', timed(k3, iters, warmup), V * 12))
 
